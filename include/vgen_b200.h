@@ -146,6 +146,16 @@ int vgen_sinusoidal_embedding(const float* t, void* out, int64_t b, int64_t dim,
 int vgen_adaptive_avgpool(const void* x, void* y, int64_t nimg, int64_t h, int64_t w, int64_t c, int64_t oh, int64_t ow,
                           int silu_in, void* stream);
 
+/* VideoComposer condition stem (cond_stem.cu): y = AdaptiveAvgPool_{oh x ow}(SiLU(conv3x3_pad1(x) + bias)) in one launch,
+ * with no full-resolution intermediate.  x [b][cin][f][h][w] (fp32 or fp16, the engines' layout), 1 <= cin <= 4;
+ * weight fp32 [cout][cin][3][3], bias fp32 [cout], cout a multiple of 8 and <= 64; y fp16 channels-last
+ * [(b f)][oh][ow][cout] (16-byte aligned).  Pooling bins are PyTorch's (start = floor(i*h/oh), end = ceil((i+1)*h/oh));
+ * fp32 accumulation, one rounding at the store.
+ * replaces: Conv2d -> SiLU -> AdaptiveAvgPool2d, the first three modules of depth / motion / canny / masked / sketch /
+ * single_sketch / local_image_embedding, unet_videolcm.py:295-372 (unet_tf2tv.py:292-369), applied at :598-703 (:594-699) */
+int vgen_cond_stem(const void* x, int x_is_f32, int64_t b, int64_t cin, int64_t f, int64_t h, int64_t w, const float* weight,
+                   const float* bias, int64_t cout, void* y, int64_t oh, int64_t ow, void* stream);
+
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */
 int vgen_vae_sample(const void* moments, const float* noise, float* z, int64_t n, int64_t zc, int64_t p, float scale,

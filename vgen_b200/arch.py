@@ -1,8 +1,8 @@
 """Architecture plans and parameter specs (names + shapes) of the UNets / VAE on the hot path.
 
 The checkpoint format IS the interface: `load_state_dict(strict=True)` must accept the reference's
-key names and shapes (1 480 tensors for UNetSD_T2VBase, 1 509 for UNetSD_I2VGen, 248 for
-AutoencoderKL).  The plan below is derived from the constructor arguments exactly as the reference
+key names and shapes (1 480 tensors for UNetSD_T2VBase, 1 509 for UNetSD_I2VGen, 1 574 for UNetSD_TFT2V /
+UNetSD_VideoLCM with the released VideoComposer compositions, 248 for AutoencoderKL).  The plan below is derived from the constructor arguments exactly as the reference
 builds its module tree:
     tools/modules/unet/unet_t2v.py:87-208, unet_i2vgen.py:88-240 (block layout),
     tools/modules/unet/util.py:311-353,674-741,807-898,1189-1238,1652-1684 (per-module parameters),
@@ -43,6 +43,8 @@ class UNetPlan:
     concat_dim: int
     use_fps_condition: bool
     context_embedding_depth: int = 0        # higen: depth of TextContextCrossTransformerMultiLayer
+    video_compositions: Tuple[str, ...] = ()  # videolcm / tft2v: config.video_compositions (condition encoders built)
+    resolution: Tuple[int, ...] = ()        # videolcm / tft2v: config.resolution [W, H]; the stems pool to (H//2, W//2)
     input_blocks: List[List[Layer]] = field(default_factory=list)
     middle: List[Layer] = field(default_factory=list)
     output_blocks: List[List[Layer]] = field(default_factory=list)
@@ -50,7 +52,8 @@ class UNetPlan:
 
 def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, num_tokens=4, dim_mult=(1, 2, 3, 4),
               num_heads=None, head_dim=64, num_res_blocks=3, attn_scales=(1 / 2, 1 / 4, 1 / 8), temporal_attention=True,
-              use_fps_condition=False, concat_dim=8, context_embedding_depth=4, **_ignored) -> UNetPlan:
+              use_fps_condition=False, concat_dim=8, context_embedding_depth=4, video_compositions=(), resolution=(),
+              **_ignored) -> UNetPlan:
     """Block layout for the given constructor kwargs (defaults are the reference's own)."""
     if not temporal_attention:
         raise NotImplementedError("temporal_attention=False is not on the sampling hot path")
@@ -65,6 +68,9 @@ def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, nu
     plan = UNetPlan(kind, in_dim, dim, embed_dim, y_dim, context_dim, out_dim, head_dim, num_tokens,
                     concat_dim if has_concat else 0, use_fps_condition,
                     context_embedding_depth if kind == "higen" else 0)
+    if kind == "videolcm":
+        plan.video_compositions = tuple(video_compositions)
+        plan.resolution = tuple(resolution or ())
     enc_dims = [dim * u for u in [1] + list(dim_mult)]
     dec_dims = [dim * u for u in [dim_mult[-1]] + list(dim_mult)[::-1]]
     shortcut = []
@@ -175,17 +181,54 @@ def _mlp(p, a, b, c):
     return _lin(p + "0.", b, a) + _lin(p + "2.", c, b)
 
 
+def _transformer_v2(p, cd):
+    """Transformer_v2 / TransformerV2(heads=2, dim=cd, dim_head=cd, mlp_dim=cd, depth=1): PreNorm attention, then
+    FeedForward(cd -> 4cd -> cd) (util.py:1396-1452, unet_videolcm.py:121-141)."""
+    e = p + "layers.0."
+    return (_norm(e + "0.norm.", cd) + _lin(e + "0.fn.to_qkv.", 2 * cd * 3, cd, False) + _lin(e + "0.fn.to_out.0.", cd, 2 * cd) +
+            _lin(e + "1.net.0.0.", cd * 4, cd) + _lin(e + "1.net.2.", cd, cd * 4))
+
+
+# VideoComposer spatial conditions of UNetSD_VideoLCM / UNetSD_TFT2V (unet_videolcm.py:295-372), in module registration
+# order: (composition name, forward keyword, encoder prefix, frame-transformer prefix, input channels).
+VCOMP_SPATIAL = (
+    ("depthmap", "depth", "depth_embedding.", "depth_embedding_after.", 1),
+    ("motion", "motion", "motion_embedding.", "motion_embedding_after.", 2),
+    ("canny", "canny", "canny_embedding.", "canny_embedding_after.", 1),
+    ("mask", "masked", "masked_embedding.", "mask_embedding_after.", 4),
+    ("sketch", "sketch", "sketch_embedding.", "sketch_embedding_after.", 1),
+    ("single_sketch", "single_sketch", "single_sketch_embedding.", "single_sketch_embedding_after.", 1),
+    ("local_image", "local_image", "local_image_embedding.", "local_image_embedding_after.", 3),
+)
+# the order in which the forward sums the encodings into `concat` (unet_videolcm.py:599-699)
+VCOMP_SUM_ORDER = ("depth", "local_image", "motion", "canny", "sketch", "single_sketch", "masked")
+VCOMP_NAMES = frozenset(["text", "image", "histogram"] + [c[0] for c in VCOMP_SPATIAL])
+
+
+def _vcomp_spec(plan: UNetPlan) -> Spec:
+    """pre_image_condition and the condition encoders, unet_videolcm.py:283-372."""
+    s: Spec = []
+    comps, cd = plan.video_compositions, plan.concat_dim
+    if "image" in comps:
+        s += _mlp("pre_image_condition.", plan.context_dim, plan.context_dim, plan.context_dim * plan.num_tokens)
+    for name, _kw, enc, after, cin in VCOMP_SPATIAL:
+        if name in comps:
+            s += _conv(enc + "0.", cd * 4, cin, 3, 3) + _conv(enc + "3.", cd * 4, cd * 4, 3, 3) + _conv(enc + "5.", cd, cd * 4, 3, 3)
+            s += _transformer_v2(after, cd)
+    return s
+
+
 def unet_spec(plan: UNetPlan) -> Spec:
     s: Spec = _mlp("time_embed.", plan.dim, plan.embed_dim, plan.embed_dim)
+    if plan.kind == "videolcm":
+        s += _vcomp_spec(plan)
     if plan.kind == "i2vgen":
         cd = plan.concat_dim
         s += _mlp("context_embedding.", plan.y_dim, plan.embed_dim, plan.context_dim * plan.num_tokens)
         s += _mlp("fps_embedding.", plan.dim, plan.embed_dim, plan.embed_dim)
         s += _conv("local_image_concat.0.", cd * 4, 4, 3, 3) + _conv("local_image_concat.2.", cd * 4, cd * 4, 3, 3) + \
             _conv("local_image_concat.4.", cd, cd * 4, 3, 3)
-        e = "local_temporal_encoder.layers.0."
-        s += _norm(e + "0.norm.", cd) + _lin(e + "0.fn.to_qkv.", 2 * cd * 3, cd, False) + _lin(e + "0.fn.to_out.0.", cd, 2 * cd)
-        s += _lin(e + "1.net.0.0.", cd * 4, cd) + _lin(e + "1.net.2.", cd, cd * 4)
+        s += _transformer_v2("local_temporal_encoder.", cd)
         s += _conv("local_image_embedding.0.", cd * 8, 4, 3, 3) + _conv("local_image_embedding.3.", cd * 16, cd * 8, 3, 3) + \
             _conv("local_image_embedding.5.", 1024, cd * 16, 3, 3)
     elif plan.use_fps_condition:

@@ -548,6 +548,26 @@ def adaptive_avgpool(x, oh, ow, silu_in=False):
     return y
 
 
+def cond_stem(x, weight, bias, oh, ow):
+    """AdaptiveAvgPool_{oh x ow}(SiLU(conv3x3_pad1(x) + bias)) of a pixel-space condition x [b, cin, f, h, w] (fp32 or
+    fp16) -> fp16 channels-last [(b f), oh, ow, cout].  weight [cout, cin, 3, 3] and bias [cout] fp32 on x's device."""
+    if not x.is_cuda or x.dim() != 5 or not x.is_contiguous() or x.dtype not in (torch.float32, torch.float16):
+        raise _l.VgenError("cond_stem: x must be a contiguous CUDA fp32/fp16 tensor [b, cin, f, h, w]")
+    b, cin, f, h, w = x.shape
+    cout = weight.shape[0]
+    if (weight.dtype != torch.float32 or not weight.is_contiguous() or weight.device != x.device
+            or tuple(weight.shape) != (cout, cin, 3, 3)):
+        raise _l.VgenError(f"cond_stem: weight must be contiguous fp32 [cout, {cin}, 3, 3] on {x.device}")
+    if bias.dtype != torch.float32 or not bias.is_contiguous() or bias.device != x.device or tuple(bias.shape) != (cout,):
+        raise _l.VgenError(f"cond_stem: bias must be contiguous fp32 [{cout}] on {x.device}")
+    y = torch.empty(b * f, oh, ow, cout, device=x.device, dtype=torch.float16)
+    rc = _run("cond_stem", 2.0 * b * f * h * w * cout * cin * 9, x.numel() * x.element_size() + y.numel() * 2,
+              lambda: _l.load().vgen_cond_stem(_p(x), 1 if x.dtype == torch.float32 else 0, b, cin, f, h, w, _p(weight),
+                                               _p(bias), cout, _p(y), oh, ow, _stream()))
+    _l.check(rc, "vgen_cond_stem")
+    return y
+
+
 def ddim_step_(xt, y, u, coef7, guide_scale, mean_type_v=True, noise=None, x0_out=None):
     """In-place fused CFG + DDIM update of the fp32 latent xt; y/u fp16 model outputs (same layout).
     x0_out (optional, fp32 like xt) receives the predicted x0 (diffusion_ddim.py:241 returns it)."""

@@ -1,7 +1,7 @@
-"""H100-native UNetSD_T2VBase / UNetSD_I2VGen / UNetSD_VideoLCM / UNetSD_SR600 / UNetSD_HiGen: same constructor
-arguments, state_dict keys and forward signatures as the reference classes (tools/modules/unet/unet_t2v.py:19-277,
-unet_i2vgen.py:19-346, unet_videolcm.py:188-760, unet_sr600.py:52-299, unet_higen.py:175-467), but the forward is a
-fixed-layout graph of libvgen_b200.so kernels.
+"""H100-native UNetSD_T2VBase / UNetSD_I2VGen / UNetSD_VideoLCM / UNetSD_TFT2V / UNetSD_SR600 / UNetSD_HiGen: same
+constructor arguments, state_dict keys and forward signatures as the reference classes (tools/modules/unet/unet_t2v.py:19-277,
+unet_i2vgen.py:19-346, unet_videolcm.py:188-760, unet_tf2tv.py:188-753, unet_sr600.py:52-299, unet_higen.py:175-467), but
+the forward is a fixed-layout graph of libvgen_b200.so kernels.
 
 Design (not a port of the reference's module tree):
   * activations stay fp16 channels-last [(b f), h, w, C] for the whole forward; the reference's dozens
@@ -90,13 +90,18 @@ class _UNetBase(SpecModule):
                                    num_tokens=num_tokens, dim_mult=tuple(dim_mult), num_heads=num_heads, head_dim=head_dim,
                                    num_res_blocks=num_res_blocks, attn_scales=tuple(attn_scales),
                                    temporal_attention=temporal_attention, use_fps_condition=use_fps_condition,
-                                   concat_dim=concat_dim, context_embedding_depth=context_embedding_depth)
+                                   concat_dim=concat_dim, context_embedding_depth=context_embedding_depth,
+                                   **self._plan_kwargs(config))
         # attributes the reference exposes and engines read
         self.in_dim, self.dim, self.y_dim, self.context_dim, self.out_dim = in_dim, dim, y_dim, context_dim, out_dim
         self.embed_dim, self.num_tokens, self.head_dim = dim * 4, num_tokens, head_dim
         self.zero_y = zero_y
         self.use_fps_condition = self.plan.use_fps_condition
         self._build_params(arch.unet_spec(self.plan), arch.unet_zero_init)
+
+    def _plan_kwargs(self, config):
+        """Extra unet_plan arguments a subclass reads from `config`."""
+        return {}
 
     # ------------------------------------------------------------------------------ weight packing
     def _pack(self):
@@ -124,6 +129,11 @@ class _UNetBase(SpecModule):
             w = sd[p + "weight"]  # [n, c, 3, 1, 1] -> [n, 3*c], k = kt*c + ci
             W[p + "w"] = _f16(w[:, :, :, 0, 0].permute(0, 2, 1).reshape(w.shape[0], -1), dev)
             W[p + "b"] = _f32(sd[p + "bias"], dev)
+
+        def transformer_v2(p):
+            e = p + "layers.0."
+            norm(e + "0.norm."), lin(e + "0.fn.to_qkv.", bias=False), lin(e + "0.fn.to_out.0.")
+            lin(e + "1.net.0.0."), lin(e + "1.net.2.")
 
         def fold(key, wmat, bias, nrm):
             """LayerNorm `nrm` folded into the linear `key` that consumes it (ops.fold_layer_norm)."""
@@ -194,10 +204,18 @@ class _UNetBase(SpecModule):
         if self.KIND == "i2vgen":
             lin("context_embedding.0."), lin("context_embedding.2.")
             conv3("local_image_concat.0.", cin_pad=8), conv3("local_image_concat.2."), conv3("local_image_concat.4.")
-            e = "local_temporal_encoder.layers.0."
-            norm(e + "0.norm."), lin(e + "0.fn.to_qkv.", bias=False), lin(e + "0.fn.to_out.0.")
-            lin(e + "1.net.0.0."), lin(e + "1.net.2.")
+            transformer_v2("local_temporal_encoder.")
             conv3("local_image_embedding.0.", cin_pad=8), conv3("local_image_embedding.3."), conv3("local_image_embedding.5.")
+        if self.KIND == "videolcm":
+            comps = self.plan.video_compositions
+            if "image" in comps:
+                lin("pre_image_condition.0."), lin("pre_image_condition.2.")
+            for name, _kw, enc, after, _cin in arch.VCOMP_SPATIAL:
+                if name in comps:
+                    # the stem conv stays fp32 [cout][cin][3][3] (ops.cond_stem); the stride-2 convs are tap-GEMM packed
+                    W[enc + "0.w"], W[enc + "0.b"] = _f32(sd[enc + "0.weight"], dev), _f32(sd[enc + "0.bias"], dev)
+                    conv3(enc + "3."), conv3(enc + "5.")
+                    transformer_v2(after)
         if self.KIND == "higen":
             W["context_embedding.tokens"] = _f16(sd["context_embedding.tokens"][0], dev)
             for d in range(self.plan.context_embedding_depth):
@@ -373,6 +391,33 @@ class _UNetBase(SpecModule):
         g = ops.group_norm(x, W["out.0.g"], W["out.0.b"], 1e-5, True)
         return ops.conv2d_3x3(g, W["out.2.w"], bias=W["out.2.b"])
 
+    def _frame_transformer(self, x, W, p, b, f):
+        """Transformer_v2 / TransformerV2(heads=2, dim=cd, dim_head=cd) over the f frames of each pixel (util.py:1396-1452,
+        unet_videolcm.py:121-141) on x [(b f), h, w, cd] -> tokens [(b f h w), cd]."""
+        n, h, w, cd = x.shape
+        e = p + "layers.0."
+        tok = x.view(-1, cd)
+        xn = ops.layer_norm(tok, W[e + "0.norm.g"], W[e + "0.norm.b"])
+        qkv = ops.linear_small(xn, W[e + "0.fn.to_qkv.w"]).view(b, f, h * w, 6 * cd)
+        att = ops.attention_temporal(qkv[..., :2 * cd], qkv[..., 2 * cd:4 * cd], qkv[..., 4 * cd:], 2, cd)
+        tok = ops.linear_small(att.view(-1, 2 * cd), W[e + "0.fn.to_out.0.w"], W[e + "0.fn.to_out.0.b"], residual=tok)
+        hid = ops.linear_small(tok, W[e + "1.net.0.0.w"], W[e + "1.net.0.0.b"], gelu_out=True)
+        return ops.linear_small(hid, W[e + "1.net.2.w"], W[e + "1.net.2.b"], residual=tok)
+
+    def _context(self, parts, b):
+        """torch.cat(parts, dim=1) of [b, L_i, context_dim] fp16 token blocks: one strided copy per part (rows = videos)."""
+        if len(parts) == 1:
+            return parts[0]
+        ltot = sum(p.shape[1] for p in parts)
+        ctx = torch.empty(b, ltot, self.context_dim, device=parts[0].device, dtype=torch.float16)
+        off, cdim = 0, self.context_dim
+        ctx_rows = ctx.view(b, ltot * cdim)
+        for part in parts:
+            lp = part.shape[1]
+            ops.copy2d(part.reshape(b, lp * cdim), ctx_rows[:, off * cdim:(off + lp) * cdim])
+            off += lp
+        return ctx
+
     def _mlp(self, x, W, p):
         h = ops.linear_small(x, W[p + "0.w"], W[p + "0.b"])
         return ops.linear_small(h, W[p + "2.w"], W[p + "2.b"], silu_in=True)
@@ -446,16 +491,8 @@ class UNetSD_I2VGen(_UNetBase):
         ximg = self._small_conv(ximg, W, "local_image_concat.0.")
         ximg = self._small_conv(ximg, W, "local_image_concat.2.", act_silu=True)
         ximg = self._small_conv(ximg, W, "local_image_concat.4.", act_silu=True)      # [(b f), h, w, cd]
-        cd = ximg.shape[-1]
-        # TransformerV2(heads=2, dim=cd, dim_head=cd): tokens are the f frames of one pixel (util.py:1396-1452)
-        e = "local_temporal_encoder.layers.0."
-        tok = ximg.view(-1, cd)
-        xn = ops.layer_norm(tok, W[e + "0.norm.g"], W[e + "0.norm.b"])
-        qkv = ops.linear_small(xn, W[e + "0.fn.to_qkv.w"]).view(b, f, h * w, 6 * cd)
-        att = ops.attention_temporal(qkv[..., :2 * cd], qkv[..., 2 * cd:4 * cd], qkv[..., 4 * cd:], 2, cd)
-        tok = ops.linear_small(att.view(-1, 2 * cd), W[e + "0.fn.to_out.0.w"], W[e + "0.fn.to_out.0.b"], residual=tok)
-        hid = ops.linear_small(tok, W[e + "1.net.0.0.w"], W[e + "1.net.0.0.b"], gelu_out=True)
-        tok = ops.linear_small(hid, W[e + "1.net.2.w"], W[e + "1.net.2.b"], residual=tok)
+        # TransformerV2(heads=2, dim=cd, dim_head=cd): tokens are the f frames of one pixel
+        tok = self._frame_transformer(ximg, W, "local_temporal_encoder.", b, f)
         return ops.eltwise("scale", tok, s=2.0)   # "concat += _ximg" twice (:294-295), exact in fp16
 
     def _local_tokens(self, local_first, W, b, h, w):
@@ -494,35 +531,74 @@ class UNetSD_I2VGen(_UNetBase):
             img = self._to_f16_rows(image).view(-1, image.shape[-1])
             ce = self._mlp(img, W, "context_embedding.")
             parts.append(ce.view(b, self.num_tokens, self.context_dim))
-        ltot = sum(p.shape[1] for p in parts)
-        ctx = torch.empty(b, ltot, self.context_dim, device=x.device, dtype=torch.float16)
-        off, cdim = 0, self.context_dim
-        ctx_rows = ctx.view(b, ltot * cdim)
-        for part in parts:                      # one strided copy per part (rows = videos)
-            lp = part.shape[1]
-            ops.copy2d(part.reshape(b, lp * cdim), ctx_rows[:, off * cdim:(off + lp) * cdim])
-            off += lp
+        ctx = self._context(parts, b)
         xin = ops.cp_to_pc(x.contiguous(), b, c, f * h * w, c_pad=c + cd).view(-1, c + cd)
         ops.copy2d(concat, xin[:, c:])
         out = self._trunk(xin.view(b * f, h, w, c + cd), emb, ctx, W, b, f)
         return ops.pc_to_cp(out.view(b, f * h * w, self.out_dim), b, self.out_dim, f * h * w).view(b, self.out_dim, f, h, w)
 
 
+def _cfg_get(config, key, default=None):
+    """config.key for the reference's EasyDict / attribute configs and for plain dicts."""
+    if config is None:
+        return default
+    if isinstance(config, dict):
+        return config.get(key, default)
+    return getattr(config, key, default)
+
+
 class UNetSD_VideoLCM(_UNetBase):
-    """Drop-in for tools/modules/unet/unet_videolcm.py:188-189 (MODEL 'UNetSD_VideoLCM') on the text-to-video
-    path of configs/videolcm_t2v_infer.yaml (video_compositions == ['text']): `concat` stays all-zero
-    (:598), pre_image is an empty Sequential (:409,:705) and the context is the text tokens (:713-726).
-    The other compositions (depth / sketch / motion / ... adapters of the VideoComposer path) are outside
-    SURVEY.md section 8 and raise."""
+    """Drop-in for tools/modules/unet/unet_videolcm.py:188-189 (MODEL 'UNetSD_VideoLCM'), text-to-video
+    (configs/videolcm_t2v_infer.yaml) and VideoComposer (videolcm_vcomposer_infer.yaml) alike.
+
+    config.video_compositions selects the condition encoders (:283-372): each spatial condition of the forward
+    ([b, cin, f, H, W] in pixel space) goes through ops.cond_stem (Conv2d + SiLU + AdaptiveAvgPool2d to
+    config.resolution / 2 in one kernel), two stride-2 convs and a Transformer_v2 over the frames; the encodings are summed
+    in the reference's order into the concat_dim channels next to x (:598-703).  'image' adds num_tokens context tokens
+    after the text tokens (pre_image_condition, :743-745).  A listed condition passed as None contributes nothing, as in
+    the reference.  'histogram' (per-frame context tokens, no released config) and config.use_text_clip_vip_model raise."""
     KIND = "videolcm"
 
     def __init__(self, config=None, *args, **kwargs):
-        comps = list(getattr(config, "video_compositions", None) or (config or {}).get("video_compositions", ["text"]))
-        if comps != ["text"]:
-            raise NotImplementedError(f"vgen_b200 UNetSD_VideoLCM: video_compositions {comps} != ['text'] is not on the hot path")
+        comps = list(_cfg_get(config, "video_compositions", None) or ["text"])
+        unknown = sorted(set(comps) - arch.VCOMP_NAMES)
+        if unknown:
+            raise ValueError(f"vgen_b200 {type(self).__name__}: unknown video_compositions {unknown}")
+        if "histogram" in comps:
+            raise NotImplementedError(f"vgen_b200 {type(self).__name__}: the 'histogram' composition (per-frame context "
+                                      "tokens) is not supported")
+        if _cfg_get(config, "use_text_clip_vip_model", False):
+            raise NotImplementedError(f"vgen_b200 {type(self).__name__}: config.use_text_clip_vip_model is not supported")
+        if "mask" in comps and not kwargs.get("inpainting", True):
+            raise NotImplementedError(f"vgen_b200 {type(self).__name__}: 'mask' with inpainting=False is not supported")
+        self._spatial = {kw: (enc, after, cin) for name, kw, enc, after, cin in arch.VCOMP_SPATIAL if name in comps}
+        res = _cfg_get(config, "resolution", None)
+        if self._spatial and (res is None or len(res) != 2):
+            raise ValueError(f"vgen_b200 {type(self).__name__}: spatial compositions need config.resolution = [W, H]")
+        self._comps, self._res = comps, tuple(res) if res is not None else ()
         super().__init__(config, *args, **kwargs)
         self.video_compositions = comps
+        self.resolution = self._res
         self.concat_dim = self.plan.concat_dim
+
+    def _plan_kwargs(self, config):
+        return dict(video_compositions=tuple(self._comps), resolution=self._res)
+
+    def _encode_condition(self, v, kw, W, b, f, h, w):
+        """<kw>_embedding + <kw>_embedding_after (unet_videolcm.py:599-699) -> tokens [(b f h w), concat_dim] fp16."""
+        enc, after, cin = self._spatial[kw]
+        if v.dim() != 5 or v.shape[0] != b or v.shape[1] != cin or v.shape[2] != f:
+            raise ValueError(f"condition '{kw}' must be [{b}, {cin}, {f}, H, W], got {list(v.shape)}")
+        if v.dtype not in (torch.float32, torch.float16):
+            v = v.float()
+        res = self.plan.resolution
+        s = ops.cond_stem(v.contiguous(), W[enc + "0.w"], W[enc + "0.b"], res[1] // 2, res[0] // 2)
+        s = self._conv3x3_s2(s, W, enc + "3.")
+        s = self._conv3x3_s2(s, W, enc + "5.", act_silu=True)                  # [(b f), h', w', cd]
+        if s.shape[1:3] != (h, w):
+            raise ValueError(f"condition '{kw}' encodes to {tuple(s.shape[1:3])} latent pixels, x has {(h, w)}: "
+                             f"config.resolution {list(res)} does not match the latent")
+        return self._frame_transformer(s, W, after, b, f)
 
     @graphed
     @torch.no_grad()
@@ -530,24 +606,47 @@ class UNetSD_VideoLCM(_UNetBase):
                 masked=None, canny=None, sketch=None, histogram=None, fps=None, video_mask=None,
                 focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0, **kwargs):
         self._check_x(x, t)
-        for name, v in (("depth", depth), ("image", image), ("motion", motion), ("local_image", local_image),
-                        ("single_sketch", single_sketch), ("masked", masked), ("canny", canny), ("sketch", sketch),
-                        ("histogram", histogram)):
-            if v is not None:
-                raise NotImplementedError(f"vgen_b200 UNetSD_VideoLCM: condition '{name}' is not on the text-only hot path")
+        name = type(self).__name__
+        if histogram is not None:
+            raise NotImplementedError(f"vgen_b200 {name}: the 'histogram' condition is not supported")
+        conds = dict(depth=depth, local_image=local_image, motion=motion, canny=canny, sketch=sketch,
+                     single_sketch=single_sketch, masked=masked)
+        for kw, v in conds.items():
+            if v is not None and kw not in self._spatial:
+                raise ValueError(f"vgen_b200 {name}: condition '{kw}' was passed but its composition is not in "
+                                 f"video_compositions {self.video_compositions}")
+        if image is not None and "image" not in self.video_compositions:
+            raise ValueError(f"vgen_b200 {name}: 'image' was passed but is not in video_compositions {self.video_compositions}")
         W = self._packed or self._pack()
         b, c, f, h, w = x.shape
+        concat = None
+        for kw in arch.VCOMP_SUM_ORDER:
+            if conds[kw] is not None:
+                e = self._encode_condition(conds[kw], kw, W, b, f, h, w)
+                concat = e if concat is None else ops.eltwise("add", concat, e)
         emb = self._time_embedding(t, fps, W)
         if y is None:
             if self.zero_y is None:
                 raise ValueError("y is None and no zero_y was given")
-            y = self.zero_y.to(x.device).repeat(b, 1, 1)            # all tokens (:724-725), unlike T2VBase
-        ctx = self._to_f16_rows(y)
-        cin = self.plan.input_blocks[0][0].cin                      # in_dim + concat_dim; the concat channels are 0
+            y = self.zero_y.to(x.device).repeat(b, 1, 1)            # all tokens (:740), unlike T2VBase
+        parts = [self._to_f16_rows(y)]
+        if image is not None:                                       # pre_image_condition(image) -> num_tokens tokens (:743-745)
+            img = self._to_f16_rows(image.reshape(b, -1, image.shape[-1]))
+            parts.append(self._mlp(img.view(-1, img.shape[-1]), W, "pre_image_condition.").view(b, self.num_tokens, self.context_dim))
+        ctx = self._context(parts, b)
+        cin = self.plan.input_blocks[0][0].cin                      # in_dim + concat_dim; the concat channels are 0 without conditions
         cpad = ((cin + 7) // 8) * 8
         xin = ops.cp_to_pc(x.contiguous(), b, c, f * h * w, c_pad=cpad).view(b * f, h, w, cpad)
+        if concat is not None:
+            ops.copy2d(concat, xin.view(-1, cpad)[:, c:c + self.concat_dim])
         out = self._trunk(xin, emb, ctx, W, b, f)
         return ops.pc_to_cp(out.view(b, f * h * w, self.out_dim), b, self.out_dim, f * h * w).view(b, self.out_dim, f, h, w)
+
+
+class UNetSD_TFT2V(UNetSD_VideoLCM):
+    """Drop-in for tools/modules/unet/unet_tf2tv.py:188-189 (MODEL 'UNetSD_TFT2V'): the VideoLCM class under TF-T2V's name.
+    The two differ only in the use_lcm / t_w arguments (unused upstream) and in y passing through misc_dropout
+    (unet_tf2tv.py:727), which is the identity in eval() (DropPath.forward :151-153); the state_dict layout is the same."""
 
 
 class UNetSD_SR600(_UNetBase):
