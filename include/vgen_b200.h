@@ -62,6 +62,23 @@ typedef struct vgen_epilogue {
 int vgen_linear(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, void* out,
                 int64_t ldo, const vgen_epilogue* epi, void* stream);
 
+/* Adapter down projection (DreamVideo, tools/modules/unet/util.py:499-519):
+ *   out[m][j] = fp16(gelu_erf(a[m][:k] . w[j][:k] + bias[j] + row_bias[m / rows_per_group][j]))
+ * with the fp32 row bias added to the fp32 accumulator before the activation (it carries the adapter's condition term
+ * lambda * down(condition_linear(c)), one row per frame or per video); bias and row_bias may be NULL.  out may be a
+ * column slice of a wider buffer (ldo), e.g. the K tail of [attn_out | h] that the fused output / up projection reads.
+ * row_bias: fp32, 8-byte aligned, even ld_row_bias >= n.  Same tap-GEMM kernels as vgen_linear (vgen_set_tapgemm_impl). */
+int vgen_linear_gelu_rowbias(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, const float* bias,
+                             const float* row_bias, int64_t ld_row_bias, int64_t rows_per_group, void* out, int64_t ldo,
+                             void* stream);
+/* The condition term of every conditioned adapter of a forward in one launch (adapter.cu):
+ *   g[r][j] = lam[r / groups_per_lam] * (c[r][:k] . w[j][:k] + v[j])      (lam NULL: lam_scalar)
+ * c fp16 [rows][k] (row stride ldc), w fp16 [n][k] = the stacked products down.W * condition_linear.W, v fp32 [n] = the
+ * stacked down.W * condition_linear.b, g fp32 [rows][n] (row stride ldg); k % 8 == 0, c / w 16-byte aligned.
+ * replaces: "x + condition_lam * self.condition_linear(condition)" ahead of down_linear, util.py:511-514 */
+int vgen_adapter_condition(const void* c, int64_t rows, int64_t k, int64_t ldc, const void* w, const float* v, int64_t n,
+                           const float* lam, float lam_scalar, int64_t groups_per_lam, float* g, int64_t ldg, void* stream);
+
 /* 3x3 / stride 1 / pad 1 conv on [nimg][h][w][c] fp16; w is [n][9*c] with k = (ky*3+kx)*c + ci.
  * replaces: nn.Conv2d in ResBlock util.py:845-876, Upsample.conv :761, head unet_t2v.py:204-207,
  *           VAE ResnetBlock / Upsample / conv_in / conv_out autoencoder.py:282-300,448-452,603,647 */

@@ -2,7 +2,8 @@
 
 The checkpoint format IS the interface: `load_state_dict(strict=True)` must accept the reference's
 key names and shapes (1 480 tensors for UNetSD_T2VBase, 1 509 for UNetSD_I2VGen, 1 574 for UNetSD_TFT2V /
-UNetSD_VideoLCM with the released VideoComposer compositions, 248 for AutoencoderKL).  The plan below is derived from the constructor arguments exactly as the reference
+UNetSD_VideoLCM with the released VideoComposer compositions, 1 850 for UNetSD_DreamVideo with the released identity and
+motion adapters, 248 for AutoencoderKL).  The plan below is derived from the constructor arguments exactly as the reference
 builds its module tree:
     tools/modules/unet/unet_t2v.py:87-208, unet_i2vgen.py:88-240 (block layout),
     tools/modules/unet/util.py:311-353,674-741,807-898,1189-1238,1652-1684 (per-module parameters),
@@ -45,6 +46,15 @@ class UNetPlan:
     context_embedding_depth: int = 0        # higen: depth of TextContextCrossTransformerMultiLayer
     video_compositions: Tuple[str, ...] = ()  # videolcm / tft2v: config.video_compositions (condition encoders built)
     resolution: Tuple[int, ...] = ()        # videolcm / tft2v: config.resolution [W, H]; the stems pool to (H//2, W//2)
+    # DreamVideo adapters (unet_dreamvideo.py:45-51): sites per transformer kind, hidden width (0: width // 2), the temporal
+    # adapters' condition width (0: none) and the position ('parallel' | 'serial') of each site
+    spatial_adapters: Tuple[str, ...] = ()
+    temporal_adapters: Tuple[str, ...] = ()
+    spatial_adapter_hidden: int = 0
+    temporal_adapter_hidden: int = 0
+    adapter_condition_dim: int = 0
+    spatial_adapter_positions: Tuple[str, ...] = ()
+    temporal_adapter_positions: Tuple[str, ...] = ()
     input_blocks: List[List[Layer]] = field(default_factory=list)
     middle: List[Layer] = field(default_factory=list)
     output_blocks: List[List[Layer]] = field(default_factory=list)
@@ -53,7 +63,8 @@ class UNetPlan:
 def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, num_tokens=4, dim_mult=(1, 2, 3, 4),
               num_heads=None, head_dim=64, num_res_blocks=3, attn_scales=(1 / 2, 1 / 4, 1 / 8), temporal_attention=True,
               use_fps_condition=False, concat_dim=8, context_embedding_depth=4, video_compositions=(), resolution=(),
-              **_ignored) -> UNetPlan:
+              spatial_adapters=(), temporal_adapters=(), spatial_adapter_hidden=0, temporal_adapter_hidden=0,
+              adapter_condition_dim=0, spatial_adapter_positions=(), temporal_adapter_positions=(), **_ignored) -> UNetPlan:
     """Block layout for the given constructor kwargs (defaults are the reference's own)."""
     if not temporal_attention:
         raise NotImplementedError("temporal_attention=False is not on the sampling hot path")
@@ -71,6 +82,11 @@ def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, nu
     if kind == "videolcm":
         plan.video_compositions = tuple(video_compositions)
         plan.resolution = tuple(resolution or ())
+    plan.spatial_adapters, plan.temporal_adapters = tuple(spatial_adapters), tuple(temporal_adapters)
+    plan.spatial_adapter_hidden, plan.temporal_adapter_hidden = spatial_adapter_hidden, temporal_adapter_hidden
+    plan.adapter_condition_dim = adapter_condition_dim
+    plan.spatial_adapter_positions = tuple(spatial_adapter_positions)
+    plan.temporal_adapter_positions = tuple(temporal_adapter_positions)
     enc_dims = [dim * u for u in [1] + list(dim_mult)]
     dec_dims = [dim * u for u in [dim_mult[-1]] + list(dim_mult)[::-1]]
     shortcut = []
@@ -142,10 +158,31 @@ def _attn(p, dim, ctx):
             _lin(p + "to_out.0.", dim, dim))
 
 
-def _basic_block(p, dim, ctx):
-    """BasicTransformerBlock registration order: attn1, ff, attn2, norm1..3 (util.py:681-696)."""
-    return (_attn(p + "attn1.", dim, dim) + _lin(p + "ff.net.0.proj.", dim * 8, dim) + _lin(p + "ff.net.2.", dim, dim * 4) +
-            _attn(p + "attn2.", dim, ctx) + _norm(p + "norm1.", dim) + _norm(p + "norm2.", dim) + _norm(p + "norm3.", dim))
+# DreamVideo adapter sites of BasicTransformerBlockWithAdapter (util.py:641-647): (list name, module name, index into the
+# position list, the output projection of the sublayer it runs next to)
+ADAPTER_SITES = (("self_attention", "attn_adapter", 0, "attn1.to_out.0."),
+                 ("cross_attention", "cross_attn_adapter", 1, "attn2.to_out.0."),
+                 ("feedforward", "ff_adapter", 2, "ff.net.2."))
+ADAPTER_NAMES = frozenset(a[0] for a in ADAPTER_SITES)
+
+
+def adapter_hidden(dim, hidden=0):
+    """Adapter hidden width (util.py:640: dim // 2 unless given)."""
+    return hidden if hidden else dim // 2
+
+
+def _basic_block(p, dim, ctx, adapters=(), hidden=0, cond_dim=0):
+    """BasicTransformerBlock registration order: attn1, ff, attn2, norm1..3 (util.py:681-696); then the DreamVideo
+    adapters in site order, each down_linear, up_linear (, condition_linear) (util.py:499-508,641-647)."""
+    s = (_attn(p + "attn1.", dim, dim) + _lin(p + "ff.net.0.proj.", dim * 8, dim) + _lin(p + "ff.net.2.", dim, dim * 4) +
+         _attn(p + "attn2.", dim, ctx) + _norm(p + "norm1.", dim) + _norm(p + "norm2.", dim) + _norm(p + "norm3.", dim))
+    h = adapter_hidden(dim, hidden)
+    for name, mod, _i, _out in ADAPTER_SITES:
+        if name in adapters:
+            s += _lin(f"{p}{mod}.down_linear.", h, dim) + _lin(f"{p}{mod}.up_linear.", dim, h)
+            if cond_dim:
+                s += _lin(f"{p}{mod}.condition_linear.", dim, cond_dim)
+    return s
 
 
 def _layer_spec(L: Layer, plan: UNetPlan) -> Spec:
@@ -166,10 +203,12 @@ def _layer_spec(L: Layer, plan: UNetPlan) -> Spec:
         # context_dim of the decoder blocks is hard-coded to 1024 upstream (unet_t2v.py:180)
         ctx = 1024 if p.startswith("output_blocks") else plan.context_dim
         return (_norm(p + "norm.", L.cin) + _lin(p + "proj_in.", L.inner, L.cin) +
-                _basic_block(p + "transformer_blocks.0.", L.inner, ctx) + _lin(p + "proj_out.", L.inner, L.cin))
+                _basic_block(p + "transformer_blocks.0.", L.inner, ctx, plan.spatial_adapters, plan.spatial_adapter_hidden) +
+                _lin(p + "proj_out.", L.inner, L.cin))
     if L.kind == "temporal":
         return (_norm(p + "norm.", L.cin) + _conv(p + "proj_in.", L.inner, L.cin, 1) +
-                _basic_block(p + "transformer_blocks.0.", L.inner, L.inner) + _conv(p + "proj_out.", L.cin, L.inner, 1))
+                _basic_block(p + "transformer_blocks.0.", L.inner, L.inner, plan.temporal_adapters, plan.temporal_adapter_hidden,
+                             plan.adapter_condition_dim) + _conv(p + "proj_out.", L.cin, L.inner, 1))
     if L.kind == "down":
         return _conv(p + "op.", L.cout, L.cin, 3, 3)
     if L.kind == "up":

@@ -13,7 +13,7 @@ static int g_tapgemm_impl = 0;  // 0 = auto (wgmma whenever C % 64 == 0, else si
 // epilogue / pipeline fill).  With FEW M tiles (the coarse levels of the UNet) the persistent grid runs
 // ceil(tiles / SMs) waves and the widest tile can leave most of the last wave idle, while a narrower one adds a wave
 // of less work each.  So the cost is waves x (BN + overhead), waves counted on this device.
-static int pick_bn(long n, int geglu, long m_tiles, int ctas) {
+static int pick_bn(long n, int geglu, long m_tiles, int ctas, int max_bn) {
   if (geglu) {
     for (int bn = 256; bn >= 64; bn -= 64)
       if (n % bn == 0) return bn;
@@ -23,7 +23,7 @@ static int pick_bn(long n, int geglu, long m_tiles, int ctas) {
   if (ctas < 1) ctas = 1;
   int best = 128;
   double best_cost = 1e30;
-  for (int bn = 256; bn >= 96; bn -= 32) {
+  for (int bn = max_bn; bn >= 96; bn -= 32) {
     const long nb = (n + bn - 1) / bn;
     const long tiles = nb * (m_tiles > 0 ? m_tiles : 1);
     const long waves = (tiles + ctas - 1) / ctas;
@@ -89,7 +89,7 @@ static int finish_and_launch(TapGemmArgs* t, const vgen_epilogue* epi, void* str
   TapGemmShape& s = t->shape;
   s.kc = s.c / 64;
   const long m_tiles_all = (long)s.d3 * cdiv(s.d2, s.box2) * cdiv(s.d1, s.box1);
-  int bn = (epi && epi->bn > 0) ? epi->bn : pick_bn(s.n, t->epi.geglu, m_tiles_all, sm_count());
+  int bn = (epi && epi->bn > 0) ? epi->bn : pick_bn(s.n, t->epi.geglu, m_tiles_all, sm_count(), t->epi.gelu ? kMaxBnGelu : 256);
   VG_REQUIRE(bn > 0, "tapgemm: no valid N tile (GEGLU needs n % 64 == 0)");
   s.bn = bn;
   s.nb = cdiv(s.n, bn);
@@ -143,6 +143,43 @@ int vgen_linear(const void* a, int64_t m, int64_t k, int64_t lda, const void* w,
   }
   VG_REQUIRE(!t.epi.group_bias, "vgen_linear: group_bias is only defined for conv entries");
   return finish_and_launch(&t, epi, stream);
+}
+
+int vgen_linear_gelu_rowbias(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, const float* bias,
+                             const float* row_bias, int64_t ld_row_bias, int64_t rows_per_group, void* out, int64_t ldo,
+                             void* stream) {
+  VG_REQUIRE(a && w && out, "vgen_linear_gelu_rowbias: null pointer");
+  VG_REQUIRE(m >= 0 && k > 0 && n > 0 && lda >= k && ldo >= n, "vgen_linear_gelu_rowbias: bad shape");
+  VG_REQUIRE(row_bias == nullptr || (rows_per_group >= 1 && rows_per_group < (1L << 31) && ld_row_bias >= n &&
+                                     ld_row_bias % 2 == 0 && (reinterpret_cast<uintptr_t>(row_bias) & 7) == 0),
+             "vgen_linear_gelu_rowbias: row_bias needs rows_per_group >= 1, an even ld_row_bias >= n and 8-byte alignment");
+  if (m == 0) return 0;
+  TapGemmArgs t{};
+  t.a = reinterpret_cast<const __half*>(a);
+  t.w = reinterpret_cast<const __half*>(w);
+  t.a_stride1 = lda;
+  t.a_stride2 = lda * m;
+  t.a_stride3 = lda * m;
+  TapGemmShape& s = t.shape;
+  s.c = (int)k;
+  s.d1 = (int)m;
+  s.d2 = 1;
+  s.d3 = 1;
+  s.box1 = 128;
+  s.box2 = 1;
+  s.num_taps = 1;
+  s.tap1[0] = s.tap2[0] = s.tap3[0] = 0;
+  s.n = (int)n;
+  TapGemmEpilogue& e = t.epi;
+  e.out = reinterpret_cast<__half*>(out);
+  e.ldo = ldo;
+  e.alpha = 1.0f;
+  e.bias = bias;
+  e.gelu = 1;
+  e.row_bias = row_bias;
+  e.ld_row_bias = row_bias ? ld_row_bias : 0;
+  e.rows_per_group = row_bias ? (int)rows_per_group : 1;
+  return finish_and_launch(&t, nullptr, stream);
 }
 
 int vgen_conv2d_3x3(const void* x, int64_t nimg, int64_t h, int64_t w_, int64_t c, const void* w, int64_t n, void* out,

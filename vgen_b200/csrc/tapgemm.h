@@ -6,6 +6,7 @@
 namespace vg {
 
 static constexpr int kMaxTaps = 9;
+static constexpr int kMaxBnGelu = 224;   // widest N tile of the GELU / row-bias epilogue (BN = 256 spills registers)
 
 // Division by a launch-time constant as multiply-high + shift (exact for 0 <= x < 2^31).  The persistent
 // kernels decompose a tile index with three div/mod pairs per tile in every warp role; with hardware
@@ -73,6 +74,11 @@ struct TapGemmEpilogue {
   int geglu;                 // out has n/2 columns: value * gelu(gate)
   const float2* row_stats;   // [rows] {rstd, -mean * rstd} or null: LayerNorm folded into the epilogue (linear only)
   const float* col_sum;      // [n]: sum_k w[n][k]   (GEGLU: indexed like bias)
+  int gelu;                  // out = gelu_erf(acc + bias + row_bias) in fp32, one rounding (adapter down projection)
+  const float* row_bias;     // [rows / rows_per_group][n] fp32 or null: added to the accumulator before the activation
+  long ld_row_bias;
+  int rows_per_group;
+  FastDiv f_rows_per_group;  // filled by the wgmma launcher
 };
 
 struct TapGemmArgs {

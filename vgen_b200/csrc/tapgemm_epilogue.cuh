@@ -102,11 +102,13 @@ __device__ __forceinline__ void epi_stage_drain(const EpiStore& st) {
 
 __device__ __forceinline__ float round_h(float x) { return __half2float(__float2half_rn(x)); }
 
-// kGeglu / kLn are template parameters of the kernel: the epilogues have very different register needs.
+// kGeglu / kLn / kGelu are template parameters of the kernel: the epilogues have very different register needs.
 // kLn: LayerNorm folded into the GEMM (TapGemmEpilogue.row_stats / col_sum): the accumulator row is scaled by the row's
 // rstd and shifted by (-mean * rstd) * col_sum[n]; such launches carry no residual / per-frame bias.
+// kGelu: adapter down projection (util.py:512-515): gelu_erf(acc + bias + row_bias[row / rows_per_group]) in fp32 and one
+// fp16 rounding at the store (the fp32 row bias carries the adapter's condition term); no residual / per-frame bias.
 // q2 = 2 * (lane % 4): this thread's column pair inside every 8-column group.
-template <int BN, bool kGeglu, bool kLn>
+template <int BN, bool kGeglu, bool kLn, bool kGelu>
 __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, const TapGemmEpilogue& e, const EpiTile& t,
                                                       EpiStore& st, bool vec_ok, int out_n, int q2, float (&acc)[BN / 2]) {
   float ln_scale[2] = {e.alpha, e.alpha}, ln_shift[2] = {0.f, 0.f};   // kLn: rstd (* alpha) and -mean * rstd of the rows
@@ -123,6 +125,12 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
   if constexpr (!kGeglu) {
     const int n0 = t.nb_i * BN;
     const __half* grow = e.group_bias ? e.group_bias + (long)fd_div(e.f_group_bias_div, t.i3) * e.ld_group_bias : nullptr;
+    const float* rrb[2] = {nullptr, nullptr};   // kGelu: this thread's rows of the row bias
+    if (kGelu && e.row_bias) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (t.row_ok[h]) rrb[h] = e.row_bias + (long)fd_div(e.f_rows_per_group, (int)t.row[h]) * e.ld_row_bias;
+    }
 #pragma unroll
     for (int c = 0; c < BN / 32; ++c) {
       const int nbase = n0 + c * 32;
@@ -159,6 +167,20 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
           if (kLn) {
             f0 = fmaf(ln_shift[h], cs.x, f0);
             f1 = fmaf(ln_shift[h], cs.y, f1);
+          }
+          if (kGelu) {
+            if (rrb[h]) {
+              if (vec) {
+                const float2 g = __ldg(reinterpret_cast<const float2*>(rrb[h] + n));
+                f0 += g.x;
+                f1 += g.y;
+              } else {
+                if (n < s.n) f0 += rrb[h][n];
+                if (n + 1 < s.n) f1 += rrb[h][n + 1];
+              }
+            }
+            f0 = gelu_erf(f0);
+            f1 = gelu_erf(f1);
           }
           if (have_g) {
             // reference: h (fp16 conv output) + emb_out (fp16) -> fp16  (util.py:909-919)

@@ -43,6 +43,8 @@ __global__ void tapgemm_simt_kernel(const __half* __restrict__ A, long st1, long
     a = dot(n) * ln_scale;
     if (e.bias) a += e.bias[n];
     if (e.row_stats) a = fmaf(ln_shift, e.col_sum[n], a);
+    if (e.row_bias) a += e.row_bias[(row / e.rows_per_group) * e.ld_row_bias + n];
+    if (e.gelu) a = gelu_erf_s(a);
     if (e.group_bias) a = __half2float(__float2half_rn(a)) + __half2float(e.group_bias[(long)(i3 / e.group_bias_div) * e.ld_group_bias + n]);
     if (e.residual) a = __half2float(__float2half_rn(a)) + __half2float(e.residual[row * e.ldr + n]);
   } else {

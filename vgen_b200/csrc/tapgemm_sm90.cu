@@ -46,13 +46,14 @@ struct alignas(64) TapGemmKernelParams {
   int stages;
 };
 
-// kEpi: bit 0 = GEGLU epilogue, bit 1 = LayerNorm folded into the epilogue (TapGemmEpilogue.row_stats); BN (the wgmma N and
-// the accumulator count) is a template parameter as well, so every register index of the epilogue is a constant.
+// kEpi: bit 0 = GEGLU epilogue, bit 1 = LayerNorm folded into the epilogue (TapGemmEpilogue.row_stats), bit 2 = GELU with the
+// fp32 row bias (TapGemmEpilogue.gelu); BN (the wgmma N and the accumulator count) is a template parameter as well, so every
+// register index of the epilogue is a constant.
 template <int BN, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_constant__ TapGemmKernelParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atom (8 rows x 128 B).
-  constexpr bool kGeglu = (kEpi & 1) != 0, kLn = (kEpi & 2) != 0;
+  constexpr bool kGeglu = (kEpi & 1) != 0, kLn = (kEpi & 2) != 0, kGelu = (kEpi & 4) != 0;
   constexpr int kBBytes = BN * kBK * 2;                            // multiple of 1024 (BN % 32 == 0)
   constexpr int kStageBytes = kABytes + kBBytes;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_
       t.row_ok[h] = (r0 + 8 * h < rows_in_tile) && (i1 < s.d1) && (i2 < s.d2);
       t.row[h] = ((long)t.i3 * s.d2 + i2) * s.d1 + i1;
     }
-    tapgemm_epilogue_tile<BN, kGeglu, kLn>(s, e, t, est, vec_ok, out_n, q2, acc);
+    tapgemm_epilogue_tile<BN, kGeglu, kLn, kGelu>(s, e, t, est, vec_ok, out_n, q2, acc);
   }
   epi_stage_drain(est);
 }
@@ -199,6 +200,8 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
   if (attr_once.need()) {
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    if constexpr (BN < 256)
+      VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if constexpr (BN % 64 == 0) {
       VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -208,6 +211,9 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
   if constexpr (BN % 64 == 0) {
     if (kind == 3) launch_kernel(tapgemm_sm90_kernel<BN, 3>, dim3(grid), dim3(kThreads), smem, stream, p);
     if (kind == 1) launch_kernel(tapgemm_sm90_kernel<BN, 1>, dim3(grid), dim3(kThreads), smem, stream, p);
+  }
+  if constexpr (BN < 256) {   // the GELU epilogue spills at BN = 256: the launcher never picks it (kMaxBnGelu)
+    if (kind == 4) launch_kernel(tapgemm_sm90_kernel<BN, 4>, dim3(grid), dim3(kThreads), smem, stream, p);
   }
   if (kind == 2) launch_kernel(tapgemm_sm90_kernel<BN, 2>, dim3(grid), dim3(kThreads), smem, stream, p);
   if (kind == 0) launch_kernel(tapgemm_sm90_kernel<BN, 0>, dim3(grid), dim3(kThreads), smem, stream, p);
@@ -227,12 +233,16 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   if (a.epi.geglu) VG_REQUIRE(s.bn % 64 == 0 && s.n % s.bn == 0, "tapgemm_sm90: GEGLU needs BN%64==0 and N%BN==0");
   if (a.epi.row_stats) VG_REQUIRE(!a.epi.residual && !a.epi.group_bias && s.num_taps == 1 && s.d2 == 1 && s.d3 == 1,
                                   "tapgemm: a folded LayerNorm goes with a plain linear (no residual / per-frame bias)");
+  if (a.epi.gelu) VG_REQUIRE(s.bn <= kMaxBnGelu, "tapgemm_sm90: the GELU epilogue needs BN <= 224");
+  if (a.epi.gelu) VG_REQUIRE(!a.epi.geglu && !a.epi.row_stats && !a.epi.residual && !a.epi.group_bias && s.num_taps == 1 &&
+                             s.d2 == 1 && s.d3 == 1, "tapgemm: the GELU / row-bias epilogue goes with a plain linear");
 
   TapGemmKernelParams p;
   p.s = s;
   tapgemm_prepare_shape(p.s);
   p.e = a.epi;
   p.e.f_group_bias_div = make_fastdiv(p.e.group_bias_div > 1 ? p.e.group_bias_div : 1);
+  p.e.f_rows_per_group = make_fastdiv(p.e.rows_per_group > 1 ? p.e.rows_per_group : 1);
   {
     const uint64_t dims[4] = {(uint64_t)s.c, (uint64_t)s.d1, (uint64_t)s.d2, (uint64_t)s.d3};
     const uint64_t strides[3] = {(uint64_t)a.a_stride1 * 2, (uint64_t)a.a_stride2 * 2, (uint64_t)a.a_stride3 * 2};
@@ -267,7 +277,7 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   int grid = sm_count();
   if (grid > s.total_tiles) grid = s.total_tiles;
   if (grid < 1) return 0;
-  const int kind = (a.epi.geglu ? 1 : 0) | (a.epi.row_stats ? 2 : 0);
+  const int kind = (a.epi.geglu ? 1 : 0) | (a.epi.row_stats ? 2 : 0) | (a.epi.gelu ? 4 : 0);
   switch (s.bn) {
     case 32: return launch_bn<32>(p, kind, grid, smem, stream);
     case 64: return launch_bn<64>(p, kind, grid, smem, stream);

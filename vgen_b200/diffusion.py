@@ -64,15 +64,22 @@ def cfg_forward(model, xt, ts, model_kwargs, by_keyword=False):
     A vgen_b200 UNet (`cfg_batch = True`) evaluates both branches as ONE forward of batch 2b -- the same arithmetic
     per sample (batch entries never interact), half the launches, and two tiles per CTA pair on the low-resolution
     layers so their epilogue overlaps a main loop.  Any other callable (e.g. a reference model) gets the reference's
-    two separate calls.  VGEN_CFG_BATCH=0 disables the batching."""
+    two separate calls.  VGEN_CFG_BATCH=0 disables the batching.
+
+    Keys a model names in `cfg_per_sample` are per-sample scalars (a number or a [b] tensor per branch, e.g. DreamVideo's
+    ag_strength): the two branches become one fp32 [2b] tensor, so branches with different values still run as one
+    forward, and one CUDA graph serves any value."""
     kc, ku = model_kwargs
     m = _unwrap(model)
     call = (lambda x, t, kw: model(x, t=t, **kw)) if by_keyword else (lambda x, t, kw: model(x, t, **kw))
     if getattr(m, "cfg_batch", False) and os.environ.get("VGEN_CFG_BATCH", "1") != "0" and kc.keys() == ku.keys():
         merged = {}
+        per_sample = getattr(m, "cfg_per_sample", ())
         for k in kc:
             a, b = kc[k], ku[k]
-            if torch.is_tensor(a) and torch.is_tensor(b) and a.shape == b.shape and a.dtype == b.dtype and a.dim() >= 1 \
+            if k in per_sample and a is not None and b is not None:
+                merged[k] = torch.cat([_per_sample(a, xt), _per_sample(b, xt)])
+            elif torch.is_tensor(a) and torch.is_tensor(b) and a.shape == b.shape and a.dtype == b.dtype and a.dim() >= 1 \
                     and a.size(0) == xt.size(0):
                 merged[k] = torch.cat([a, b], dim=0)
             elif a is None and b is None:
@@ -85,6 +92,14 @@ def cfg_forward(model, xt, ts, model_kwargs, by_keyword=False):
             n = xt.size(0)
             return out[:n], out[n:]
     return call(xt, ts, kc), call(xt, ts, ku)
+
+
+def _per_sample(v, xt):
+    """A number or a 1- / b-entry tensor -> fp32 [b] on xt's device (b = xt.size(0))."""
+    t = torch.as_tensor(v, dtype=torch.float32).to(xt.device).reshape(-1)
+    if t.numel() not in (1, xt.size(0)):
+        raise ValueError(f"a per-sample argument must be a number or have {xt.size(0)} entries, got {t.numel()}")
+    return t.expand(xt.size(0))
 
 
 class DiffusionDDIM(object):

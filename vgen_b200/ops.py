@@ -147,6 +147,62 @@ def linear(a, w, bias=None, residual=None, alpha=1.0, geglu=False, out=None, bn=
     return out
 
 
+def linear_gelu_rowbias(a, w, bias=None, row_bias=None, rows_per_group=1, out=None):
+    """out[m, j] = fp16(gelu_erf(a[m] . w[j] + bias[j] + row_bias[m // rows_per_group, j])): the adapter down projection.
+    The fp32 row bias [groups, n] (a row-strided 2-D view is fine) is added to the fp32 accumulator before the activation;
+    `a` and `out` may be row-strided 2-D views (out e.g. the K tail of the buffer the fused up projection reads)."""
+    _chk16(a, "a"), _chk16(w, "w")
+    a2, lda = _rows_view(a, "a")
+    m, k = a2.shape
+    n = w.shape[0]
+    if w.shape[1] != k or not w.is_contiguous():
+        raise _l.VgenError(f"linear_gelu_rowbias: weight {tuple(w.shape)} does not match k={k}")
+    if bias is not None and (bias.dtype != torch.float32 or not bias.is_contiguous() or bias.numel() != n):
+        raise _l.VgenError(f"linear_gelu_rowbias: bias must be contiguous fp32 [{n}]")
+    ldg = 0
+    if row_bias is not None:
+        if (row_bias.dtype != torch.float32 or row_bias.dim() != 2 or row_bias.shape[1] != n or row_bias.stride(1) != 1
+                or row_bias.device != a.device):
+            raise _l.VgenError(f"linear_gelu_rowbias: row_bias must be fp32 [groups, {n}] with contiguous rows on {a.device}")
+        if rows_per_group < 1 or row_bias.shape[0] * rows_per_group < m:
+            raise _l.VgenError(f"linear_gelu_rowbias: {row_bias.shape[0]} row-bias rows x {rows_per_group} do not cover {m} rows")
+        ldg = row_bias.stride(0)
+    if out is None:
+        out = torch.empty(m, n, device=a.device, dtype=torch.float16)
+    o2, ldo = _rows_view(out, "out")
+    if tuple(o2.shape) != (m, n):
+        raise _l.VgenError(f"linear_gelu_rowbias: out is {tuple(o2.shape)}, expected {(m, n)}")
+    rc = _run("tapgemm", 2.0 * m * n * k, 2.0 * (m * k + n * k + m * n),
+              lambda: _l.load().vgen_linear_gelu_rowbias(_p(a2), m, k, lda, _p(w), n, _p(bias), _p(row_bias), ldg,
+                                                         int(rows_per_group), _p(o2), ldo, _stream()),
+              tag=f"adapter down m{m} k{k} n{n}")
+    _l.check(rc, "vgen_linear_gelu_rowbias")
+    return out
+
+
+def adapter_condition(c, w, v, lam=None, lam_scalar=1.0, groups_per_lam=1):
+    """g[r, j] = lam[r // groups_per_lam] * (c[r] . w[j] + v[j]) as fp32 [rows, n]: the condition term of every conditioned
+    adapter at once (w / v: the stacked down.W @ condition_linear.W / down.W @ condition_linear.b).  lam: fp32 [groups]
+    on the device, or None for lam_scalar."""
+    _chk16(c, "c"), _chk16(w, "w")
+    c2, ldc = _rows_view(c, "c")
+    rows, k = c2.shape
+    n = w.shape[0]
+    if w.shape[1] != k or not w.is_contiguous():
+        raise _l.VgenError(f"adapter_condition: weight {tuple(w.shape)} does not match k={k}")
+    if v.dtype != torch.float32 or not v.is_contiguous() or v.numel() != n:
+        raise _l.VgenError(f"adapter_condition: v must be contiguous fp32 [{n}]")
+    if lam is not None and (lam.dtype != torch.float32 or not lam.is_contiguous() or lam.device != c.device
+                            or lam.numel() * groups_per_lam < rows):
+        raise _l.VgenError("adapter_condition: lam must be a contiguous fp32 tensor on c's device with one entry per group")
+    g = torch.empty(rows, n, device=c.device, dtype=torch.float32)
+    rc = _run("adapter_condition", 2.0 * rows * n * k, 2.0 * (rows * k + n * k) + 4.0 * rows * n,
+              lambda: _l.load().vgen_adapter_condition(_p(c2), rows, k, ldc, _p(w), _p(v), n, _p(lam), float(lam_scalar),
+                                                       int(groups_per_lam), _p(g), n, _stream()))
+    _l.check(rc, "vgen_adapter_condition")
+    return g
+
+
 def conv2d_3x3(x, w, bias=None, group_bias=None, residual=None, out=None, bn=0, group_div=1):
     """x [nimg, h, w, c] fp16 -> [nimg, h, w, n]; w [n, 9*c] with k = (ky*3+kx)*c + ci."""
     _chk16(x, "x"), _chk16(w, "w")

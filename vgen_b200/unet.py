@@ -1,6 +1,7 @@
-"""H100-native UNetSD_T2VBase / UNetSD_I2VGen / UNetSD_VideoLCM / UNetSD_TFT2V / UNetSD_SR600 / UNetSD_HiGen: same
-constructor arguments, state_dict keys and forward signatures as the reference classes (tools/modules/unet/unet_t2v.py:19-277,
-unet_i2vgen.py:19-346, unet_videolcm.py:188-760, unet_tf2tv.py:188-753, unet_sr600.py:52-299, unet_higen.py:175-467), but
+"""H100-native UNetSD_T2VBase / UNetSD_I2VGen / UNetSD_VideoLCM / UNetSD_TFT2V / UNetSD_DreamVideo / UNetSD_SR600 /
+UNetSD_HiGen: same constructor arguments, state_dict keys and forward signatures as the reference classes
+(tools/modules/unet/unet_t2v.py:19-277, unet_i2vgen.py:19-346, unet_videolcm.py:188-760, unet_tf2tv.py:188-753,
+unet_dreamvideo.py:19-290, unet_sr600.py:52-299, unet_higen.py:175-467), but
 the forward is a fixed-layout graph of libvgen_b200.so kernels.
 
 Design (not a port of the reference's module tree):
@@ -64,6 +65,7 @@ class _UNetBase(SpecModule):
     # the extra per-column terms in their epilogue; the balance has not been measured on the H100.  VGEN_LN_FOLD=1, or
     # FOLD_LN = True on a module followed by invalidate_packed(), turns it on; parity is the same (tests/test_gpu_parity.py).
     FOLD_LN = os.environ.get("VGEN_LN_FOLD", "0") == "1"
+    _adapter_rows = None   # DreamVideo: (fp32 condition terms [groups, sum of hidden widths], frames per group) of the running forward
 
     def __init__(self, config=None, in_dim=4, dim=512, y_dim=512, context_dim=512, hist_dim=156, dim_condition=4,
                  out_dim=6, num_tokens=4, dim_mult=[1, 2, 3, 4], num_heads=None, head_dim=64, num_res_blocks=3,
@@ -175,6 +177,39 @@ class _UNetBase(SpecModule):
                 W[p + "ff.geglu.cs"] = _f32(W[p + "ff.geglu.w"].double().sum(1), dev)
             lin(p + "ff.net.2.")
 
+        cond_w, cond_v = [], []   # conditioned adapters: stacked down.W @ condition_linear.W / down.W @ condition_linear.b
+
+        def adapters(q, names, positions):
+            """DreamVideo adapters of the block at q (util.py:499-519,649-670).  The hidden width is padded to a multiple of 64
+            (zero rows of down, zero columns of up) so every adapter GEMM takes the wgmma path.  Parallel: the sublayer's output
+            projection and the up projection become one GEMM over the concatenated K [W_out | W_up] with b_out + b_up.  The
+            condition term is composed here: down(x + lam (Wc c + bc)) = down(x) + lam (Wd Wc c + Wd bc)."""
+            for name, mod, idx, out in arch.ADAPTER_SITES:
+                if name not in names:
+                    continue
+                a = q + mod + "."
+                wd, bd = sd[a + "down_linear.weight"].detach().double().cpu(), sd[a + "down_linear.bias"].detach().double().cpu()
+                wu, bu = sd[a + "up_linear.weight"].detach().double().cpu(), sd[a + "up_linear.bias"].detach().double().cpu()
+                hid, c = wd.shape
+                hp = ((hid + 63) // 64) * 64
+                wd_p, bd_p, wu_p = torch.zeros(hp, c, dtype=torch.float64), torch.zeros(hp, dtype=torch.float64), \
+                    torch.zeros(c, hp, dtype=torch.float64)
+                wd_p[:hid], bd_p[:hid], wu_p[:, :hid] = wd, bd, wu
+                ad = {"pos": positions[idx], "hp": hp, "down.w": _f16(wd_p, dev), "down.b": _f32(bd_p, dev), "off": None}
+                if positions[idx] == "parallel":
+                    wo = sd[q + out + "weight"].detach().double().cpu()
+                    W[q + out + "w"] = _f16(torch.cat([wo, wu_p], dim=1), dev)
+                    W[q + out + "b"] = _f32(sd[q + out + "bias"].detach().double().cpu() + bu, dev)
+                else:
+                    ad["up.w"], ad["up.b"] = _f16(wu_p, dev), _f32(bu, dev)
+                if a + "condition_linear.weight" in sd:
+                    wc = sd[a + "condition_linear.weight"].detach().double().cpu()
+                    bc = sd[a + "condition_linear.bias"].detach().double().cpu()
+                    ad["off"] = sum(m.shape[0] for m in cond_w)
+                    cond_w.append(torch.cat([wd @ wc, torch.zeros(hp - hid, wc.shape[1], dtype=torch.float64)]))
+                    cond_v.append(torch.cat([wd @ bc, torch.zeros(hp - hid, dtype=torch.float64)]))
+                W[q + mod] = ad
+
         def layer(L):
             p = L.prefix
             if L.kind == "conv_in":
@@ -190,8 +225,10 @@ class _UNetBase(SpecModule):
                     norm(q + "0."), tconv(f"{q}{widx}.")
             elif L.kind == "spatial":
                 norm(p + "norm."), lin(p + "proj_in."), block(p + "transformer_blocks.0.", True), lin(p + "proj_out.")
+                adapters(p + "transformer_blocks.0.", self.plan.spatial_adapters, self.plan.spatial_adapter_positions)
             elif L.kind == "temporal":
                 norm(p + "norm."), lin(p + "proj_in."), block(p + "transformer_blocks.0.", False), lin(p + "proj_out.")
+                adapters(p + "transformer_blocks.0.", self.plan.temporal_adapters, self.plan.temporal_adapter_positions)
             elif L.kind == "down":
                 conv3(p + "op.")
             elif L.kind == "up":
@@ -233,6 +270,8 @@ class _UNetBase(SpecModule):
             for L in blk:
                 layer(L)
         norm("out.0."), conv3("out.2.")
+        if cond_w:
+            W["adapter.cond.w"], W["adapter.cond.v"] = _f16(torch.cat(cond_w), dev), _f32(torch.cat(cond_v), dev)
         self._packed = W
         return W
 
@@ -291,30 +330,59 @@ class _UNetBase(SpecModule):
             return ops.linear(t, W[key], bias=W[key + ".lb"], ln=(ops.row_stats(t), W[key + ".cs"]))
         return ops.linear(ops.layer_norm(t, W[nrm + "g"], W[nrm + "b"]), W[key])
 
-    def _self_attn_spatial(self, t, W, p, nrm, heads, n, hw, inner):
+    def _self_attn_qkv_spatial(self, t, W, p, nrm, n, hw, inner):
         qkv = self._ln_linear(t, W, p + "qkv", nrm)             # [M, 3*inner]
         v3 = qkv.view(n, hw, 3 * inner)
-        return ops.attention_d64(v3[:, :, :inner], v3[:, :, inner:2 * inner], v3[:, :, 2 * inner:], heads)
+        return v3[:, :, :inner], v3[:, :, inner:2 * inner], v3[:, :, 2 * inner:]
+
+    def _sublayer_out(self, t, W, p, mod, out, width, hw, produce):
+        """t + sublayer(t) through the output projection W[p + out]; produce(buf) writes the sublayer's [M, width] input of
+        that projection into the 2-D view buf (or returns a new tensor when buf is None).  With a DreamVideo adapter at
+        p + mod (util.py:649-670) the parallel form is ONE GEMM [sublayer | h] . [W_out | W_up]^T + (b_out + b_up) + t, h =
+        gelu(down(t) + condition term) written into the K tail of the same buffer; the serial form adds up(h(t')) + t' to
+        t' = t + sublayer(t).  Without one it is the plain projection with the residual."""
+        ad = W.get(p + mod)
+        if ad is None:
+            return ops.linear(produce(None).view(-1, width), W[p + out + "w"], bias=W[p + out + "b"], residual=t)
+        if ad["pos"] == "serial":
+            t = ops.linear(produce(None).view(-1, width), W[p + out + "w"], bias=W[p + out + "b"], residual=t)
+            h = self._adapter_down(t, ad, hw)
+            return ops.linear(h, ad["up.w"], bias=ad["up.b"], residual=t)
+        buf = torch.empty(t.shape[0], width + ad["hp"], device=t.device, dtype=torch.float16)
+        produce(buf[:, :width])
+        self._adapter_down(t, ad, hw, out=buf[:, width:])
+        return ops.linear(buf, W[p + out + "w"], bias=W[p + out + "b"], residual=t)
+
+    def _adapter_down(self, t, ad, hw, out=None):
+        """gelu(down(x + lam condition_linear(c))) of Adapter.forward (util.py:510-515) in one GEMM: the condition term is the
+        fp32 row bias of this forward's adapter_condition launch (one row per video or per frame)."""
+        g = None
+        cond = self._adapter_rows
+        if ad["off"] is not None and cond is not None:
+            g = cond[0][:, ad["off"]:ad["off"] + ad["hp"]]
+        return ops.linear_gelu_rowbias(t, ad["down.w"], bias=ad["down.b"], row_bias=g,
+                                       rows_per_group=(cond[1] * hw if g is not None else 1), out=out)
 
     def _basic_block_spatial(self, t, ctx_tokens, W, p, heads, n, hw, inner, f):
         """BasicTransformerBlock on tokens t [M, inner] (M = n*hw); ctx_tokens [b, L, ctx_dim] fp16."""
-        a = self._self_attn_spatial(t, W, p + "attn1.", p + "norm1.", heads, n, hw, inner)
-        t = ops.linear(a.view(-1, inner), W[p + "attn1.to_out.0.w"], bias=W[p + "attn1.to_out.0.b"], residual=t)
+        t = self._sublayer_out(t, W, p, "attn_adapter", "attn1.to_out.0.", inner, hw, lambda o: ops.attention_d64(
+            *self._self_attn_qkv_spatial(t, W, p + "attn1.", p + "norm1.", n, hw, inner), heads,
+            out=None if o is None else o.view(n, hw, inner)))
         q = self._ln_linear(t, W, p + "attn2.q", p + "norm2.").view(n, hw, inner)
         bctx, lctx, cdim = ctx_tokens.shape
         kv = ops.linear(ctx_tokens.view(-1, cdim), W[p + "attn2.kv"]).view(bctx, lctx, 2 * inner)
-        a = ops.attention_d64(q, kv[:, :, :inner], kv[:, :, inner:], heads, kv_batch_div=f)
-        t = ops.linear(a.view(-1, inner), W[p + "attn2.to_out.0.w"], bias=W[p + "attn2.to_out.0.b"], residual=t)
-        return self._feed_forward(t, W, p)
+        t = self._sublayer_out(t, W, p, "cross_attn_adapter", "attn2.to_out.0.", inner, hw, lambda o: ops.attention_d64(
+            q, kv[:, :, :inner], kv[:, :, inner:], heads, kv_batch_div=f, out=None if o is None else o.view(n, hw, inner)))
+        return self._feed_forward(t, W, p, hw)
 
-    def _feed_forward(self, t, W, p):
-        if p + "ff.geglu.cs" in W:   # norm3 folded into the GEGLU projection
-            gg = ops.linear(t, W[p + "ff.geglu.w"], bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"],
-                            ln=(ops.row_stats(t), W[p + "ff.geglu.cs"]))
-        else:
+    def _feed_forward(self, t, W, p, hw=1):
+        def geglu(out):
+            if p + "ff.geglu.cs" in W:   # norm3 folded into the GEGLU projection
+                return ops.linear(t, W[p + "ff.geglu.w"], bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"],
+                                  ln=(ops.row_stats(t), W[p + "ff.geglu.cs"]), out=out)
             xn = ops.layer_norm(t, W[p + "norm3.g"], W[p + "norm3.b"])
-            gg = ops.linear(xn, W[p + "ff.geglu.w"], bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"])
-        return ops.linear(gg, W[p + "ff.net.2.w"], bias=W[p + "ff.net.2.b"], residual=t)
+            return ops.linear(xn, W[p + "ff.geglu.w"], bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"], out=out)
+        return self._sublayer_out(t, W, p, "ff_adapter", "ff.net.2.", W[p + "ff.geglu.w"].shape[0] // 2, hw, geglu)
 
     def _spatial_transformer(self, x, ctx_tokens, L, W, f):
         """SpatialTransformer.forward, use_linear=True (util.py:354-373)."""
@@ -326,10 +394,11 @@ class _UNetBase(SpecModule):
         out = ops.linear(t, W[p + "proj_out.w"], bias=W[p + "proj_out.b"], residual=x.view(-1, c))
         return out.view(n, h, w, c)
 
-    def _temporal_attn(self, t, W, p, nrm, heads, b, f, hw, inner):
+    def _temporal_attn(self, t, W, p, nrm, heads, b, f, hw, inner, out=None):
         qkv = self._ln_linear(t, W, p + "qkv", nrm).view(b, f, hw, 3 * inner)
         # all videos of the batch in one launch
-        return ops.attention_temporal(qkv[..., :inner], qkv[..., inner:2 * inner], qkv[..., 2 * inner:], heads, 64)
+        return ops.attention_temporal(qkv[..., :inner], qkv[..., inner:2 * inner], qkv[..., 2 * inner:], heads, 64,
+                                      out=None if out is None else out.view(b, f, hw, inner))
 
     def _temporal_transformer(self, x, L, W, b, f):
         """TemporalTransformer.forward, only_self_att=True (util.py:1240-1286): both attentions are
@@ -342,10 +411,10 @@ class _UNetBase(SpecModule):
         g = ops.group_norm(x, W[p + "norm.g"], W[p + "norm.b"], 1e-6, False, n=b)
         t = ops.linear(g.view(-1, c), W[p + "proj_in.w"], bias=W[p + "proj_in.b"])
         q = p + "transformer_blocks.0."
-        for att, nrm in (("attn1.", "norm1."), ("attn2.", "norm2.")):
-            a = self._temporal_attn(t, W, q + att, q + nrm, L.heads, b, f, hw, inner)
-            t = ops.linear(a.view(-1, inner), W[q + att + "to_out.0.w"], bias=W[q + att + "to_out.0.b"], residual=t)
-        t = self._feed_forward(t, W, q)
+        for att, nrm, mod in (("attn1.", "norm1.", "attn_adapter"), ("attn2.", "norm2.", "cross_attn_adapter")):
+            t = self._sublayer_out(t, W, q, mod, att + "to_out.0.", inner, hw, lambda o, t=t, att=att, nrm=nrm: self._temporal_attn(
+                t, W, q + att, q + nrm, L.heads, b, f, hw, inner, out=o))
+        t = self._feed_forward(t, W, q, hw)
         out = ops.linear(t, W[p + "proj_out.w"], bias=W[p + "proj_out.b"], residual=x.view(-1, c))
         return out.view(n, h, w, c)
 
@@ -647,6 +716,97 @@ class UNetSD_TFT2V(UNetSD_VideoLCM):
     """Drop-in for tools/modules/unet/unet_tf2tv.py:188-189 (MODEL 'UNetSD_TFT2V'): the VideoLCM class under TF-T2V's name.
     The two differ only in the use_lcm / t_w arguments (unused upstream) and in y passing through misc_dropout
     (unet_tf2tv.py:727), which is the identity in eval() (DropPath.forward :151-153); the state_dict layout is the same."""
+
+
+class UNetSD_DreamVideo(_UNetBase):
+    """Drop-in for tools/modules/unet/unet_dreamvideo.py:19-20 (MODEL 'UNetSD_DreamVideo', every configs/dreamvideo UNet):
+    the T2V trunk with DreamVideo's adapters (Adapter, util.py:499-519) in the transformer blocks.
+
+      * spatial_adapter_list: identity adapters of the SpatialTransformers, without condition (util.py:385-442);
+      * temporal_adapter_list: motion adapters of the TemporalTransformers, conditioned on y_image (the CLIP image embedding,
+        [b, 1, C] repeated over the frames or [b, f, C]) scaled by ag_strength when temporal_adapter_condition_dim is set.
+
+    Each adapted sublayer costs one extra launch (the down projection with GELU and the condition term, ops.linear_gelu_rowbias);
+    the up projection is fused into the sublayer's output projection.  The condition terms of all adapters come from one
+    launch per forward (ops.adapter_condition).  ag_strength may be a float or a [b] tensor; the CFG sampler merges the
+    engine's two floats into one tensor (cfg_per_sample) so the pair runs as one batch-2b forward.  With no adapters the
+    state_dict and the forward are UNetSD_T2VBase's."""
+    KIND = "t2v"
+    cfg_per_sample = ("ag_strength",)
+
+    def __init__(self, config=None, *args, spatial_adapter_list=[], spatial_adapter_position_list=["", "parallel", ""],
+                 spatial_adapter_hidden_dim=None, temporal_adapter_list=[],
+                 temporal_adapter_position_list=["parallel", "parallel", "parallel"], temporal_adapter_condition_dim=None,
+                 temporal_adapter_hidden_dim=None, **kwargs):
+        name = type(self).__name__
+        for kind, names, positions in (("spatial", spatial_adapter_list, spatial_adapter_position_list),
+                                       ("temporal", temporal_adapter_list, temporal_adapter_position_list)):
+            unknown = sorted(set(names) - arch.ADAPTER_NAMES)
+            if unknown:
+                raise ValueError(f"vgen_b200 {name}: unknown {kind} adapters {unknown} (known: {sorted(arch.ADAPTER_NAMES)})")
+            for site, _mod, idx, _out in arch.ADAPTER_SITES:
+                if site in names and (idx >= len(positions) or positions[idx] not in ("parallel", "serial")):
+                    # the reference skips the whole sublayer then (util.py:649-670): a graph change, not swallowed
+                    raise NotImplementedError(f"vgen_b200 {name}: {kind} adapter '{site}' at position "
+                                              f"{positions[idx] if idx < len(positions) else None!r}: only 'parallel' and "
+                                              "'serial' are supported")
+        self._adapter_kwargs = dict(
+            spatial_adapters=tuple(spatial_adapter_list), temporal_adapters=tuple(temporal_adapter_list),
+            spatial_adapter_hidden=int(spatial_adapter_hidden_dim or 0), temporal_adapter_hidden=int(temporal_adapter_hidden_dim or 0),
+            adapter_condition_dim=int(temporal_adapter_condition_dim or 0) if temporal_adapter_list else 0,
+            spatial_adapter_positions=tuple(spatial_adapter_position_list), temporal_adapter_positions=tuple(temporal_adapter_position_list))
+        super().__init__(config, *args, **kwargs)
+        self.spatial_adapter_list, self.temporal_adapter_list = list(spatial_adapter_list), list(temporal_adapter_list)
+        self.temporal_adapter_condition_dim = temporal_adapter_condition_dim
+
+    def _plan_kwargs(self, config):
+        return dict(self._adapter_kwargs)
+
+    def _condition_rows(self, y_image, ag_strength, b, f):
+        """Shape checks of y_image / ag_strength (before any device work).  -> (y_image as [b * fi, C], fi) or None when the
+        motion adapters take no condition (no condition dim, or y_image is None: then y_image is ignored, as upstream)."""
+        cdim = self.plan.adapter_condition_dim
+        if not cdim or y_image is None:
+            return None
+        if y_image.dim() != 3 or y_image.shape[0] != b or y_image.shape[1] not in (1, f) or y_image.shape[2] != cdim:
+            raise ValueError(f"y_image must be [{b}, 1, {cdim}] or [{b}, {f}, {cdim}], got {list(y_image.shape)}")
+        if torch.is_tensor(ag_strength) and ag_strength.numel() not in (1, b):
+            raise ValueError(f"ag_strength must be a number or have one entry per batch element ({b}), got "
+                             f"{list(ag_strength.shape)}")
+        return y_image, y_image.shape[1]
+
+    @graphed
+    @torch.no_grad()
+    def forward(self, x, t, y=None, y_image=None, fps=None, masked=None, video_mask=None, focus_present_mask=None,
+                prob_focus_present=0., mask_last_frame_num=0, ag_strength=1, **kwargs):
+        self._check_x(x, t)
+        b, c, f, h, w = x.shape
+        cond = self._condition_rows(y_image, ag_strength, b, f)
+        W = self._packed or self._pack()
+        emb = self._time_embedding(t, fps, W)
+        if y is None:
+            if self.zero_y is None:
+                raise ValueError("y is None and no zero_y was given")
+            y = self.zero_y.to(x.device).repeat(b, 1, 1)[:, :1, :]
+        ctx = self._to_f16_rows(y)
+        rows = None
+        if cond is not None and "adapter.cond.w" in W:
+            yi, fi = cond
+            c16 = self._to_f16_rows(yi).view(b * fi, yi.shape[-1])
+            if torch.is_tensor(ag_strength):
+                lam = ag_strength.to(device=x.device, dtype=torch.float32).reshape(-1).contiguous()
+                g = ops.adapter_condition(c16, W["adapter.cond.w"], W["adapter.cond.v"], lam=lam,
+                                          groups_per_lam=fi if lam.numel() == b else b * fi)
+            else:
+                g = ops.adapter_condition(c16, W["adapter.cond.w"], W["adapter.cond.v"], lam_scalar=float(ag_strength))
+            rows = (g, f // fi)                                 # one row per video (fi = 1) or per frame
+        xin = ops.cp_to_pc(x.contiguous(), b, c, f * h * w, c_pad=8).view(b * f, h, w, 8)
+        self._adapter_rows = rows
+        try:
+            out = self._trunk(xin, emb, ctx, W, b, f)                 # [(b f), h, w, out_dim]
+        finally:
+            self._adapter_rows = None
+        return ops.pc_to_cp(out.view(b, f * h * w, self.out_dim), b, self.out_dim, f * h * w).view(b, self.out_dim, f, h, w)
 
 
 class UNetSD_SR600(_UNetBase):
