@@ -3,7 +3,7 @@
 The checkpoint format IS the interface: `load_state_dict(strict=True)` must accept the reference's
 key names and shapes (1 480 tensors for UNetSD_T2VBase, 1 509 for UNetSD_I2VGen, 1 574 for UNetSD_TFT2V /
 UNetSD_VideoLCM with the released VideoComposer compositions, 1 850 for UNetSD_DreamVideo with the released identity and
-motion adapters, 248 for AutoencoderKL).  The plan below is derived from the constructor arguments exactly as the reference
+motion adapters, 2 008 for UNetSD_LoRA with InstructVideo's rank-4 LoRA, 248 for AutoencoderKL).  The plan below is derived from the constructor arguments exactly as the reference
 builds its module tree:
     tools/modules/unet/unet_t2v.py:87-208, unet_i2vgen.py:88-240 (block layout),
     tools/modules/unet/util.py:311-353,674-741,807-898,1189-1238,1652-1684 (per-module parameters),
@@ -55,6 +55,8 @@ class UNetPlan:
     adapter_condition_dim: int = 0
     spatial_adapter_positions: Tuple[str, ...] = ()
     temporal_adapter_positions: Tuple[str, ...] = ()
+    # InstructVideo LoRA (unet_lora.py:114-159): rank of the q / k / v / out LoRA pairs of every UNet attention (0: none)
+    lora_rank: int = 0
     input_blocks: List[List[Layer]] = field(default_factory=list)
     middle: List[Layer] = field(default_factory=list)
     output_blocks: List[List[Layer]] = field(default_factory=list)
@@ -64,7 +66,8 @@ def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, nu
               num_heads=None, head_dim=64, num_res_blocks=3, attn_scales=(1 / 2, 1 / 4, 1 / 8), temporal_attention=True,
               use_fps_condition=False, concat_dim=8, context_embedding_depth=4, video_compositions=(), resolution=(),
               spatial_adapters=(), temporal_adapters=(), spatial_adapter_hidden=0, temporal_adapter_hidden=0,
-              adapter_condition_dim=0, spatial_adapter_positions=(), temporal_adapter_positions=(), **_ignored) -> UNetPlan:
+              adapter_condition_dim=0, spatial_adapter_positions=(), temporal_adapter_positions=(), lora_rank=0,
+              **_ignored) -> UNetPlan:
     """Block layout for the given constructor kwargs (defaults are the reference's own)."""
     if not temporal_attention:
         raise NotImplementedError("temporal_attention=False is not on the sampling hot path")
@@ -87,6 +90,7 @@ def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, nu
     plan.adapter_condition_dim = adapter_condition_dim
     plan.spatial_adapter_positions = tuple(spatial_adapter_positions)
     plan.temporal_adapter_positions = tuple(temporal_adapter_positions)
+    plan.lora_rank = int(lora_rank)
     enc_dims = [dim * u for u in [1] + list(dim_mult)]
     dec_dims = [dim * u for u in [dim_mult[-1]] + list(dim_mult)[::-1]]
     shortcut = []
@@ -153,9 +157,19 @@ def _conv(p, n, c, *ks):
     return [(p + "weight", (n, c) + tuple(ks)), (p + "bias", (n,))]
 
 
-def _attn(p, dim, ctx):
-    return (_lin(p + "to_q.", dim, dim, False) + _lin(p + "to_k.", dim, ctx, False) + _lin(p + "to_v.", dim, ctx, False) +
-            _lin(p + "to_out.0.", dim, dim))
+# InstructVideo LoRA pairs of MemoryEfficientCrossAttention (unet_lora.py:155-159), in registration order: (LoRA module,
+# the projection it is merged into).  Each is down_linear [rank, in] then up_linear [out, rank], both without bias.
+LORA_SITES = (("to_q_lora", "to_q.weight"), ("to_k_lora", "to_k.weight"), ("to_v_lora", "to_v.weight"),
+              ("to_out_lora", "to_out.0.weight"))
+
+
+def _attn(p, dim, ctx, lora_rank=0):
+    s = (_lin(p + "to_q.", dim, dim, False) + _lin(p + "to_k.", dim, ctx, False) + _lin(p + "to_v.", dim, ctx, False) +
+         _lin(p + "to_out.0.", dim, dim))
+    if lora_rank:
+        for (mod, _w), k in zip(LORA_SITES, (dim, ctx, ctx, dim)):
+            s += _lin(f"{p}{mod}.down_linear.", lora_rank, k, False) + _lin(f"{p}{mod}.up_linear.", dim, lora_rank, False)
+    return s
 
 
 # DreamVideo adapter sites of BasicTransformerBlockWithAdapter (util.py:641-647): (list name, module name, index into the
@@ -171,11 +185,13 @@ def adapter_hidden(dim, hidden=0):
     return hidden if hidden else dim // 2
 
 
-def _basic_block(p, dim, ctx, adapters=(), hidden=0, cond_dim=0):
+def _basic_block(p, dim, ctx, adapters=(), hidden=0, cond_dim=0, lora_rank=0):
     """BasicTransformerBlock registration order: attn1, ff, attn2, norm1..3 (util.py:681-696); then the DreamVideo
-    adapters in site order, each down_linear, up_linear (, condition_linear) (util.py:499-508,641-647)."""
-    s = (_attn(p + "attn1.", dim, dim) + _lin(p + "ff.net.0.proj.", dim * 8, dim) + _lin(p + "ff.net.2.", dim, dim * 4) +
-         _attn(p + "attn2.", dim, ctx) + _norm(p + "norm1.", dim) + _norm(p + "norm2.", dim) + _norm(p + "norm3.", dim))
+    adapters in site order, each down_linear, up_linear (, condition_linear) (util.py:499-508,641-647).  With a LoRA rank
+    each attention ends with its four LoRA pairs (unet_lora.py:148-159)."""
+    s = (_attn(p + "attn1.", dim, dim, lora_rank) + _lin(p + "ff.net.0.proj.", dim * 8, dim) +
+         _lin(p + "ff.net.2.", dim, dim * 4) + _attn(p + "attn2.", dim, ctx, lora_rank) + _norm(p + "norm1.", dim) +
+         _norm(p + "norm2.", dim) + _norm(p + "norm3.", dim))
     h = adapter_hidden(dim, hidden)
     for name, mod, _i, _out in ADAPTER_SITES:
         if name in adapters:
@@ -203,12 +219,13 @@ def _layer_spec(L: Layer, plan: UNetPlan) -> Spec:
         # context_dim of the decoder blocks is hard-coded to 1024 upstream (unet_t2v.py:180)
         ctx = 1024 if p.startswith("output_blocks") else plan.context_dim
         return (_norm(p + "norm.", L.cin) + _lin(p + "proj_in.", L.inner, L.cin) +
-                _basic_block(p + "transformer_blocks.0.", L.inner, ctx, plan.spatial_adapters, plan.spatial_adapter_hidden) +
+                _basic_block(p + "transformer_blocks.0.", L.inner, ctx, plan.spatial_adapters, plan.spatial_adapter_hidden,
+                             lora_rank=plan.lora_rank) +
                 _lin(p + "proj_out.", L.inner, L.cin))
     if L.kind == "temporal":
         return (_norm(p + "norm.", L.cin) + _conv(p + "proj_in.", L.inner, L.cin, 1) +
                 _basic_block(p + "transformer_blocks.0.", L.inner, L.inner, plan.temporal_adapters, plan.temporal_adapter_hidden,
-                             plan.adapter_condition_dim) + _conv(p + "proj_out.", L.cin, L.inner, 1))
+                             plan.adapter_condition_dim, plan.lora_rank) + _conv(p + "proj_out.", L.cin, L.inner, 1))
     if L.kind == "down":
         return _conv(p + "op.", L.cout, L.cin, 3, 3)
     if L.kind == "up":
@@ -303,6 +320,8 @@ def unet_zero_init(name: str) -> bool:
         return True
     if name.startswith(("asim_embedding.2.", "msim_embedding.2.", "img_embedding.")):
         return True  # unet_higen.py:276-289
+    if name.endswith("_lora.up_linear.weight"):
+        return True  # unet_lora.py:122
     return name == "out.2.weight" or name.startswith("fps_embedding.2.")
 
 

@@ -218,6 +218,34 @@ class FrozenOpenCLIPEmbedder(_EmbedderBase):
     encode = forward
 
 
+class FrozenOpenCLIPEmbedderZero(FrozenOpenCLIPEmbedder):
+    """clip_embedder.py:230-300 (InstructVideo's embedder): forward(text) is the same text tower as FrozenOpenCLIPEmbedder.
+    The reference's white_image, zero_feature and forward_image (image features for reward training) need the visual tower
+    and are not provided: they raise NotImplementedError.  The inference entrance reads zero_feature once without using it
+    (inference_instructvideo_entrance.py:145); INTEGRATION.md says to drop that line."""
+
+    def __init__(self, pretrained, vit_resolution=(224, 224), arch="ViT-H-14", device="cuda", max_length=77, freeze=True,
+                 layer="last"):
+        super().__init__(pretrained=pretrained, vit_resolution=vit_resolution, arch=arch, device=device,
+                         max_length=max_length, freeze=freeze, layer=layer)
+
+    @staticmethod
+    def _training_only(name):
+        raise NotImplementedError(f"vgen_b200 FrozenOpenCLIPEmbedderZero.{name}: the image features of InstructVideo's reward "
+                                  "training are not provided (text tower only)")
+
+    @property
+    def white_image(self):
+        self._training_only("white_image")
+
+    @property
+    def zero_feature(self):
+        self._training_only("zero_feature")
+
+    def forward_image(self, image):
+        self._training_only("forward_image")
+
+
 class FrozenOpenCLIPVisualEmbedder(_EmbedderBase):
     """clip_embedder.py:80-143: image embedding only."""
     TEXT = False

@@ -8,8 +8,9 @@ Host side (kept in fp64 torch / Python exactly like the reference, so it is bit-
   * the timestep list  (1 + arange(0, T, T // S)).clamp(0, T-1).flip(0)   diffusion_ddim.py:250
 Only the sampling entry points used by the inference engines are provided: ddim_sample_loop and ddim_sample for
 var_type fixed_small / mean_type v|eps.  The arithmetic of the reference's p_mean_variance (:147-206: two model calls,
-CFG mix, v -> x0) has no method of its own here -- it lives inside the fused step kernel; the training losses, PLMS and
-reward variants are out of scope and absent (calling them raises AttributeError, not a fallback).
+CFG mix, v -> x0) has no method of its own here -- it lives inside the fused step kernel; the training losses and PLMS are
+out of scope and absent (calling them raises AttributeError, not a fallback).  DiffusionDDIMReward (InstructVideo) samples
+like DiffusionDDIM; its reward fine-tuning methods raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -203,3 +204,28 @@ class DiffusionDDIM(object):
             # the step index is known on the host: no device->host read of t inside the loop
             xt, _ = self._ddim_step(xt, int(step), t, model, model_kwargs, guide_scale, ddim_timesteps, eta)
         return xt
+
+
+class DiffusionDDIMReward(DiffusionDDIM):
+    """Drop-in for diffusion_ddim.py:516 (DIFFUSION 'DiffusionDDIMReward', every configs/instructvideo Diffusion): the
+    reference class inherits ddim_sample_loop unchanged and only adds gradient-carrying methods for InstructVideo's reward
+    fine-tuning.  Sampling is DiffusionDDIM's; those methods raise NotImplementedError."""
+
+    def _reward_training(self, name):
+        raise NotImplementedError(f"vgen_b200 DiffusionDDIMReward.{name}: reward fine-tuning is not supported (the native "
+                                  "path samples without gradients); use the reference class to train")
+
+    def ddim_sample_loop_partial(self, *args, **kwargs):
+        self._reward_training("ddim_sample_loop_partial")
+
+    def ddim_sample_gradient(self, *args, **kwargs):
+        self._reward_training("ddim_sample_gradient")
+
+    def ddim_sample_with_logprob(self, *args, **kwargs):
+        self._reward_training("ddim_sample_with_logprob")
+
+    def ddim_sample_loop_with_logprob(self, *args, **kwargs):
+        self._reward_training("ddim_sample_loop_with_logprob")
+
+    def loss(self, *args, **kwargs):
+        self._reward_training("loss")

@@ -58,16 +58,17 @@ USING_REFERENCE_REGISTRY = False
 
 
 def register(force_local: bool = False):
-    """Register the UNets (T2VBase, I2VGen, VideoLCM, TFT2V, DreamVideo, SR600, HiGen), DiffusionDDIM(SR), AutoencoderKL and the three
-    FrozenOpenCLIP*Embedder classes under the reference's registry names.  Returns (MODEL, DIFFUSION, AUTO_ENCODER); the
-    embedder registry is `vgen_b200.registry.EMBEDDER`."""
+    """Register the UNets (T2VBase, I2VGen, VideoLCM, TFT2V, DreamVideo, LoRA, SR600, HiGen), DiffusionDDIM(SR / Reward),
+    AutoencoderKL and the four FrozenOpenCLIP*Embedder classes under the reference's registry names.  Returns (MODEL,
+    DIFFUSION, AUTO_ENCODER); the embedder registry is `vgen_b200.registry.EMBEDDER`."""
     global MODEL, DIFFUSION, AUTO_ENCODER, EMBEDDER, USING_REFERENCE_REGISTRY
     from .autoencoder import AutoencoderKL
-    from .clip import FrozenOpenCLIPEmbedder, FrozenOpenCLIPTextVisualEmbedder, FrozenOpenCLIPVisualEmbedder
-    from .diffusion import DiffusionDDIM
+    from .clip import (FrozenOpenCLIPEmbedder, FrozenOpenCLIPEmbedderZero, FrozenOpenCLIPTextVisualEmbedder,
+                       FrozenOpenCLIPVisualEmbedder)
+    from .diffusion import DiffusionDDIM, DiffusionDDIMReward
     from .diffusion_gauss import DiffusionDDIMSR
-    from .unet import (UNetSD_DreamVideo, UNetSD_HiGen, UNetSD_I2VGen, UNetSD_SR600, UNetSD_T2VBase, UNetSD_TFT2V,
-                       UNetSD_VideoLCM)
+    from .unet import (UNetSD_DreamVideo, UNetSD_HiGen, UNetSD_I2VGen, UNetSD_LoRA, UNetSD_SR600, UNetSD_T2VBase,
+                       UNetSD_TFT2V, UNetSD_VideoLCM)
 
     regs = None
     emb = None
@@ -91,12 +92,15 @@ def register(force_local: bool = False):
                                         "the reference's (utils.registry_class)" if USING_REFERENCE_REGISTRY else "local mirror")
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")  # replacing the reference classes is the point
-        for cls in (UNetSD_T2VBase, UNetSD_I2VGen, UNetSD_VideoLCM, UNetSD_TFT2V, UNetSD_DreamVideo, UNetSD_SR600, UNetSD_HiGen):
+        for cls in (UNetSD_T2VBase, UNetSD_I2VGen, UNetSD_VideoLCM, UNetSD_TFT2V, UNetSD_DreamVideo, UNetSD_LoRA, UNetSD_SR600,
+                    UNetSD_HiGen):
             MODEL.register_class()(cls)
         DIFFUSION.register_class()(DiffusionDDIM)
         DIFFUSION.register_class()(DiffusionDDIMSR)
+        DIFFUSION.register_class()(DiffusionDDIMReward)
         AUTO_ENCODER.register_class()(AutoencoderKL)
         EMBEDDER = emb if emb is not None else (EMBEDDER or Registry("EMBEDDER"))   # also reachable as vgen_b200.registry.EMBEDDER
-        for cls in (FrozenOpenCLIPEmbedder, FrozenOpenCLIPVisualEmbedder, FrozenOpenCLIPTextVisualEmbedder):
+        for cls in (FrozenOpenCLIPEmbedder, FrozenOpenCLIPVisualEmbedder, FrozenOpenCLIPTextVisualEmbedder,
+                    FrozenOpenCLIPEmbedderZero):
             EMBEDDER.register_class()(cls)
     return MODEL, DIFFUSION, AUTO_ENCODER

@@ -1,7 +1,7 @@
-"""H100-native UNetSD_T2VBase / UNetSD_I2VGen / UNetSD_VideoLCM / UNetSD_TFT2V / UNetSD_DreamVideo / UNetSD_SR600 /
-UNetSD_HiGen: same constructor arguments, state_dict keys and forward signatures as the reference classes
+"""H100-native UNetSD_T2VBase / UNetSD_I2VGen / UNetSD_VideoLCM / UNetSD_TFT2V / UNetSD_DreamVideo / UNetSD_LoRA /
+UNetSD_SR600 / UNetSD_HiGen: same constructor arguments, state_dict keys and forward signatures as the reference classes
 (tools/modules/unet/unet_t2v.py:19-277, unet_i2vgen.py:19-346, unet_videolcm.py:188-760, unet_tf2tv.py:188-753,
-unet_dreamvideo.py:19-290, unet_sr600.py:52-299, unet_higen.py:175-467), but
+unet_dreamvideo.py:19-290, unet_lora.py:1091-1409, unet_sr600.py:52-299, unet_higen.py:175-467), but
 the forward is a fixed-layout graph of libvgen_b200.so kernels.
 
 Design (not a port of the reference's module tree):
@@ -106,8 +106,12 @@ class _UNetBase(SpecModule):
         return {}
 
     # ------------------------------------------------------------------------------ weight packing
+    def _pack_state_dict(self):
+        """The state dict the packed weights are built from (UNetSD_LoRA: with the LoRA merged in)."""
+        return {k: v for k, v in self.state_dict().items()}
+
     def _pack(self):
-        sd = {k: v for k, v in self.state_dict().items()}
+        sd = self._pack_state_dict()
         dev = self.device
         if dev.type != "cuda":
             raise ops._l.VgenError("vgen_b200 UNet forward needs the module on a CUDA device (no CPU path exists)")
@@ -806,6 +810,76 @@ class UNetSD_DreamVideo(_UNetBase):
             out = self._trunk(xin, emb, ctx, W, b, f)                 # [(b f), h, w, out_dim]
         finally:
             self._adapter_rows = None
+        return ops.pc_to_cp(out.view(b, f * h * w, self.out_dim), b, self.out_dim, f * h * w).view(b, self.out_dim, f, h, w)
+
+
+class UNetSD_LoRA(_UNetBase):
+    """Drop-in for tools/modules/unet/unet_lora.py:1091-1409 (MODEL 'UNetSD_LoRA', every configs/instructvideo UNet): the
+    T2V trunk whose attentions carry InstructVideo's LoRA pairs, q = to_q(x) + up(down(x)) and the same for k, v and out
+    (:161-195).  The state_dict keeps the LoRA pairs (2 008 tensors at the released rank 4, 1 480 without LoRA), so strict
+    loading and get_lora_merged_model (inference_instructvideo_entrance.py:301-353) work unchanged.
+
+    The forward never runs the pairs: the pack folds each one into the projection it adapts, W + s * up @ down with
+    s = lora_alpha / lora_rank (1 when lora_alpha is None), the merge the reference's inference performs, computed in fp64
+    on the host and rounded to the masters' dtype (merged_state_dict).  The packed weights are then exactly
+    UNetSD_T2VBase's for the merged dict, and the LoRA costs nothing per step.  fps is ignored and y is required, as in the
+    reference (:1315-1316)."""
+    KIND = "t2v"
+
+    def __init__(self, in_dim=7, dim=512, y_dim=512, context_dim=512, out_dim=6, dim_mult=[1, 2, 3, 4], num_heads=None,
+                 head_dim=64, num_res_blocks=3, attn_scales=[1 / 2, 1 / 4, 1 / 8], use_scale_shift_norm=True, dropout=0.1,
+                 temporal_attn_times=1, temporal_attention=True, use_checkpoint=False, use_image_dataset=False,
+                 use_fps_condition=False, use_sim_mask=False, training=True, inpainting=True, use_lora=False, lora_rank=None,
+                 lora_alpha=None):
+        if use_lora and (lora_rank is None or int(lora_rank) < 1):
+            raise ValueError(f"vgen_b200 UNetSD_LoRA: use_lora=True needs lora_rank >= 1, got {lora_rank!r}")
+        self._lora_rank = int(lora_rank) if use_lora else 0
+        super().__init__(None, in_dim=in_dim, dim=dim, y_dim=y_dim, context_dim=context_dim, out_dim=out_dim,
+                         dim_mult=dim_mult, num_heads=num_heads, head_dim=head_dim, num_res_blocks=num_res_blocks,
+                         attn_scales=attn_scales, use_scale_shift_norm=use_scale_shift_norm, dropout=dropout,
+                         temporal_attn_times=temporal_attn_times, temporal_attention=temporal_attention,
+                         use_checkpoint=use_checkpoint, use_image_dataset=use_image_dataset,
+                         use_fps_condition=use_fps_condition, use_sim_mask=use_sim_mask, training=training,
+                         inpainting=inpainting)
+        self.use_lora, self.lora_rank, self.lora_alpha = use_lora, lora_rank, lora_alpha
+        # get_lora_merged_model's alpha (inference_instructvideo_entrance.py:315)
+        self.lora_scale = lora_alpha / lora_rank if (lora_alpha is not None and self._lora_rank) else 1.0
+
+    def _plan_kwargs(self, config):
+        return dict(lora_rank=self._lora_rank)
+
+    def merged_state_dict(self):
+        """state_dict() with every LoRA pair folded into its projection (W + lora_scale * up @ down in fp64, rounded to W's
+        dtype) and the LoRA keys dropped: the UNetSD_T2VBase / use_lora=False layout.  Without LoRA it is state_dict()."""
+        sd = self.state_dict()
+        if not self.plan.lora_rank:
+            return dict(sd)
+        targets = dict(arch.LORA_SITES)
+        out = {k: v for k, v in sd.items() if "_lora." not in k}
+        for k, down in sd.items():
+            if not k.endswith("_lora.down_linear.weight"):
+                continue
+            att, mod = k[:-len(".down_linear.weight")].rsplit(".", 1)
+            w, up = sd[f"{att}.{targets[mod]}"], sd[k.replace(".down_linear.", ".up_linear.")]
+            delta = up.detach().double().cpu() @ down.detach().double().cpu()
+            out[f"{att}.{targets[mod]}"] = (w.detach().double().cpu() + self.lora_scale * delta).to(device=w.device, dtype=w.dtype)
+        return out
+
+    def _pack_state_dict(self):
+        return self.merged_state_dict()
+
+    @graphed
+    @torch.no_grad()
+    def forward(self, x, t, y, fps=None, video_mask=None, focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0):
+        self._check_x(x, t)
+        if y is None:
+            raise ValueError("UNetSD_LoRA.forward needs y (the reference has no zero_y fallback)")
+        W = self._packed or self._pack()
+        b, c, f, h, w = x.shape
+        emb = self._time_embedding(t, None, W)                        # fps is ignored (unet_lora.py:1315)
+        ctx = self._to_f16_rows(y)
+        xin = ops.cp_to_pc(x.contiguous(), b, c, f * h * w, c_pad=8).view(b * f, h, w, 8)
+        out = self._trunk(xin, emb, ctx, W, b, f)                     # [(b f), h, w, out_dim]
         return ops.pc_to_cp(out.view(b, f * h * w, self.out_dim), b, self.out_dim, f * h * w).view(b, self.out_dim, f, h, w)
 
 

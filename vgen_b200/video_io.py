@@ -1,5 +1,6 @@
-"""Video write-out (SURVEY.md section 8f-3): drop-ins for utils/video_op.py:167-213 `save_i2vgen_video_safe` and
-:263-309 `save_t2vhigen_video_safe` that take the decoded video WHERE IT IS -- on the GPU.
+"""Video write-out (SURVEY.md section 8f-3): drop-ins for utils/video_op.py:167-213 `save_i2vgen_video_safe`,
+:263-309 `save_t2vhigen_video_safe` and :216-262 `save_video_local` (InstructVideo) that take the decoded video WHERE IT
+IS -- on the GPU.
 
 The reference copies [1,3,f,H,W] fp32 to the host (173 MB at config 2), un-normalises / clamps / scales / transposes /
 casts on the CPU, and hands uint8 frames to imageio (libx264).  Here one kernel (vgen_video_to_rgb8) produces the
@@ -58,11 +59,11 @@ def select_frames(host, hband):
     return f
 
 
-def _encode(local_path, frames, save_fps):
-    """frames: uint8 numpy [n,h,w,3] RGB."""
+def _encode(local_path, frames, save_fps, video=False):
+    """frames: uint8 numpy [n,h,w,3] RGB.  One frame is written as a PNG unless `video` asks for the video file anyway."""
     n, h, w, _ = frames.shape
     os.makedirs(os.path.dirname(os.path.abspath(local_path)), exist_ok=True)
-    if n == 1:
+    if n == 1 and not video:
         import cv2
         cv2.imwrite(local_path + ".png", frames[0][:, :, ::-1], [int(cv2.IMWRITE_JPEG_QUALITY), 100])
         return local_path + ".png"
@@ -137,3 +138,26 @@ def save_i2vgen_video_safe(local_path, gen_video, captions=None, mean=[0.5, 0.5,
 
 
 save_t2vhigen_video_safe = save_i2vgen_video_safe   # identical body in the reference (:263-309)
+
+
+@torch.no_grad()
+def save_video_local(local_path, gen_video, mean=[0.5, 0.5, 0.5], std=[0.5, 0.5, 0.5], retry=5):
+    """utils/video_op.py:216-262 (InstructVideo's writer, same signature): the frames of batch entry 0 with the same
+    arithmetic as save_i2vgen_video_safe but no last-frame drop, written to local_path as an 8 fps mp4 (libx264, crf 17,
+    yuv420p) even for a single frame.  Returns the f frames as uint8 numpy [h, w, 3] RGB, like the reference.
+    gen_video is not modified (the reference un-normalises it in place).  The InstructVideo entrance passes a host tensor
+    (gen_videos.cpu(), inference_instructvideo_entrance.py:264); it is copied to the current CUDA device, where the
+    frames are made -- passing the CUDA tensor saves the round trip."""
+    if not gen_video.is_cuda:
+        gen_video = gen_video.to(torch.device("cuda", torch.cuda.current_device()))
+    host, _band, ev = frames_to_host(gen_video, mean, std)
+    ev.synchronize()
+    frames = host.numpy().copy()
+    exc = None
+    for _ in range(max(1, retry)):
+        try:
+            _encode(local_path, frames, 8, video=True)
+            return list(frames)
+        except Exception as e:  # noqa: BLE001 - retried like the reference (:241-257)
+            exc = e
+    raise exc
