@@ -123,9 +123,10 @@ int vgen_attention_d64(const void* q, const void* k, const void* v, void* out, i
  * replaces: AttnBlock.forward of the SD VAE, autoencoder.py:365-389 (w_ = bmm(q,k) * c**-0.5; softmax; bmm(v, w_)) */
 int vgen_attention_d512(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t lq, int64_t lk,
                         int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, float scale, void* stream);
-/* Per-pixel attention over L <= 32 frames (attn_temporal.cu, register-resident mma.sync): token t of
- * sequence s lives at q + s*seq_stride + t*tok_stride (+ head*head_dim).  head_dim 64 is the fast path;
- * any head_dim <= 64, L <= 64 is served by a scalar kernel (I2VGen's 4-channel local encoder).
+/* Per-pixel attention over any number L of frames (attn_temporal.cu, mma.sync): token t of
+ * sequence s lives at q + s*seq_stride + t*tok_stride (+ head*head_dim).  head_dim 64 is the fast path:
+ * register-resident for L <= 32, flash-style (K/V streamed in 64-key blocks, online softmax) for L > 32;
+ * any other head_dim <= 64 is served by a scalar kernel (the 4- and 8-channel frame transformers).
  * Videos back to back in one launch: sequence s is pixel (s % seqs_per_batch) of video (s / seqs_per_batch), whose
  * base is q + video*batch_stride (seqs_per_batch <= 0: one video, batch strides ignored).
  * replaces: memory_efficient_attention in TemporalTransformer util.py:1258-1261; Attention util.py:1396-1424 */

@@ -1,13 +1,19 @@
-// Temporal self-attention: sequences are the f (<= 32) frames of one pixel, head_dim 64.  There are
-// tens of thousands of tiny (L x L) problems per call, so a 64-row wgmma tile would be >85% padding;
-// instead each warp owns one (pixel, head) and keeps the whole problem in registers with
-// mma.sync.m16n8k16 (the S accumulator layout IS the A-fragment layout of the P V product).
-// The kernel is bound by its q/k/v reads (8 FLOP/B), not by the math.
+// Temporal self-attention: sequences are the f frames of one pixel, head_dim 64.  There are
+// tens of thousands of short (L x L) problems per call, so a 64-row wgmma tile would be mostly padding
+// (at least half at f <= 32, up to 48% at 33-63 frames); both kernels below use mma.sync.m16n8k16 fragments
+// instead (the S accumulator layout IS the A-fragment layout of the P V product).
+//  * f <= 32: attn_temporal_kernel, each warp owns one (pixel, head) and keeps the whole problem in registers.
+//    It is bound by its q/k/v reads (8 FLOP/B), not by the math.
+//  * f > 32: attn_temporal_flash_kernel, one CTA per (pixel, head, 64-query tile), each warp 16 query rows;
+//    K/V stream through shared memory in 64-key blocks (cp.async, double-buffered when f > 64) with an online
+//    softmax, so shared memory is fixed and any f works.
 //
 // Replaces xformers.ops.memory_efficient_attention for the TemporalTransformer blocks
 // (/root/reference/tools/modules/unet/util.py:231-269 called from :1258-1261, tokens '(b h w) f c');
 // the activations stay in the frame-major [f][hw][C] layout, the kernel gathers the f tokens of a pixel
 // with a stride instead of materialising the reference's '(b h w) f c' permutation.
+#include <algorithm>
+
 #include "common.h"
 #include "ptx.cuh"
 
@@ -184,8 +190,181 @@ __global__ void __launch_bounds__(128) attn_temporal_kernel(const __half* __rest
   }
 }
 
-// Generic tiny attention (any head_dim <= 64, L <= 64), one thread per (seq, head, query): used only
-// for the 4-channel local temporal encoder of UNetSD_I2VGen (unet_i2vgen.py:122-124, util.py:1396-1424).
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  // src-size 0 reads nothing and zero-fills the 16 bytes (rows past L)
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Any L > 32.  grid (nseq*heads, ceil(L/64)); blockDim 32 * ceil(min(L,64)/16).  smem: Q [64][kRow], then
+// nbuf (1 when L <= 64, else 2) K/V block pairs [64][kRow].  Warps whose 16 rows all lie past L still load and
+// meet the barriers but skip the math.
+__global__ void __launch_bounds__(128) attn_temporal_flash_kernel(
+    const __half* __restrict__ q, const __half* __restrict__ k, const __half* __restrict__ v, __half* __restrict__ out,
+    int heads, int L, long tok_stride_q, long seq_stride_q, long tok_stride_o, long seq_stride_o, float scale_log2,
+    long spb, long batch_stride_q, long batch_stride_o) {
+  constexpr int kRow = 72;
+  constexpr int kBlk = 64;
+  extern __shared__ __align__(16) __half sm_f[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nthr = blockDim.x;
+  const long item = blockIdx.x;  // (seq, head)
+  const long seq = item / heads;
+  const int head = (int)(item % heads);
+  const int q0 = blockIdx.y * kBlk;
+  const int nblk = (L + kBlk - 1) / kBlk;
+  __half* sQ = sm_f;
+  __half* sKV = sQ + kBlk * kRow;  // buffer i: K at sKV + 2*i*kBlk*kRow, V right after
+  const long vid = seq / spb, pix = seq - vid * spb;
+  const long base = vid * batch_stride_q + pix * seq_stride_q + head * 64;
+
+  for (int i = threadIdx.x; i < kBlk * 8; i += nthr) {
+    const int t = i >> 3, piece = i & 7;
+    const bool ok = q0 + t < L;
+    cp_async16(smem_u32(sQ + t * kRow + piece * 8), q + base + (ok ? (long)(q0 + t) * tok_stride_q + piece * 8 : 0), ok);
+  }
+  auto load_kv = [&](int blk, int buf) {
+    __half* sK = sKV + (size_t)buf * 2 * kBlk * kRow;
+    __half* sV = sK + kBlk * kRow;
+    for (int i = threadIdx.x; i < kBlk * 8; i += nthr) {
+      const int t = i >> 3, piece = i & 7, key = blk * kBlk + t;
+      const bool ok = key < L;
+      const long off = base + (ok ? (long)key * tok_stride_q + piece * 8 : 0);
+      cp_async16(smem_u32(sK + t * kRow + piece * 8), k + off, ok);
+      cp_async16(smem_u32(sV + t * kRow + piece * 8), v + off, ok);
+    }
+    cp_async_commit();
+  };
+  load_kv(0, 0);
+
+  const int g = lane >> 2, tq = lane & 3;
+  const int row0 = warp * 16;
+  const bool active = q0 + row0 < L;  // warp-uniform
+  uint32_t qa[4][4];
+  float o[8][4];
+#pragma unroll
+  for (int n = 0; n < 8; ++n)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) o[n][e] = 0.f;
+  float mx0 = -INFINITY, mx1 = -INFINITY, l0 = 0.f, l1 = 0.f;  // rows g and g+8 (this thread's quad-partial sums)
+
+  for (int blk = 0; blk < nblk; ++blk) {
+    if (blk + 1 < nblk) {
+      load_kv(blk + 1, (blk + 1) & 1);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (active) {
+      const __half* sK = sKV + (size_t)(blk & 1) * 2 * kBlk * kRow;
+      const __half* sV = sK + kBlk * kRow;
+      if (blk == 0) {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+          ldsm_x4(smem_u32(sQ + (row0 + (lane & 15)) * kRow + ks * 16 + ((lane >> 4) << 3)), qa[ks][0], qa[ks][1], qa[ks][2],
+                  qa[ks][3]);
+      }
+      // ---- S = Q K^T for this key block: 8 n-tiles of 8 keys
+      float s[8][4];
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) s[n][e] = 0.f;
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int n2 = 0; n2 < 4; ++n2) {
+          uint32_t b0, b1, b2, b3;
+          const int row = n2 * 16 + (lane & 7) + ((lane >> 4) << 3);
+          const int col = ks * 16 + (((lane >> 3) & 1) << 3);
+          ldsm_x4(smem_u32(sK + row * kRow + col), b0, b1, b2, b3);
+          mma16816(s[2 * n2], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b0, b1);
+          mma16816(s[2 * n2 + 1], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b2, b3);
+        }
+      }
+      // ---- online softmax: mask keys >= L, rescale the running sum and O by exp2((old max - new max) * scale)
+      float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+      for (int n = 0; n < 8; ++n) {
+        const int key = blk * kBlk + n * 8 + 2 * tq;
+        if (key >= L) s[n][0] = s[n][2] = -INFINITY;
+        if (key + 1 >= L) s[n][1] = s[n][3] = -INFINITY;
+        bm0 = fmaxf(bm0, fmaxf(s[n][0], s[n][1]));
+        bm1 = fmaxf(bm1, fmaxf(s[n][2], s[n][3]));
+      }
+      bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
+      bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+      bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
+      bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+      const float nm0 = fmaxf(mx0, bm0), nm1 = fmaxf(mx1, bm1);  // finite: key blk*64 < L is never masked
+      const float c0 = fast_exp2((mx0 - nm0) * scale_log2), c1 = fast_exp2((mx1 - nm1) * scale_log2);
+      mx0 = nm0;
+      mx1 = nm1;
+      l0 *= c0;
+      l1 *= c1;
+#pragma unroll
+      for (int n = 0; n < 8; ++n) {
+        o[n][0] *= c0;
+        o[n][1] *= c0;
+        o[n][2] *= c1;
+        o[n][3] *= c1;
+      }
+      uint32_t pa[8][2];
+#pragma unroll
+      for (int n = 0; n < 8; ++n) {
+        const float e0 = fast_exp2((s[n][0] - nm0) * scale_log2);
+        const float e1 = fast_exp2((s[n][1] - nm0) * scale_log2);
+        const float e2 = fast_exp2((s[n][2] - nm1) * scale_log2);
+        const float e3 = fast_exp2((s[n][3] - nm1) * scale_log2);
+        l0 += e0 + e1;
+        l1 += e2 + e3;
+        pa[n][0] = pack_half2(e0, e1);
+        pa[n][1] = pack_half2(e2, e3);
+      }
+      // ---- O += P V: k over the block's 64 keys (4 steps), n over d (8 tiles)
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int n2 = 0; n2 < 4; ++n2) {
+          uint32_t b0, b1, b2, b3;
+          const int row = ks * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
+          const int col = n2 * 16 + ((lane >> 4) << 3);
+          ldsm_x4_t(smem_u32(sV + row * kRow + col), b0, b1, b2, b3);
+          mma16816(o[2 * n2], pa[2 * ks][0], pa[2 * ks][1], pa[2 * ks + 1][0], pa[2 * ks + 1][1], b0, b1);
+          mma16816(o[2 * n2 + 1], pa[2 * ks][0], pa[2 * ks][1], pa[2 * ks + 1][0], pa[2 * ks + 1][1], b2, b3);
+        }
+      }
+    }
+    __syncthreads();  // the next iteration's load overwrites this buffer
+  }
+  if (!active) return;
+  // ---- normalise once, stage through this warp's own Q rows, coalesced 16-byte stores of rows < L
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+#pragma unroll
+  for (int n = 0; n < 8; ++n) {
+    const int col = n * 8 + 2 * tq;
+    *reinterpret_cast<uint32_t*>(sQ + (row0 + g) * kRow + col) = pack_half2(o[n][0] * i0, o[n][1] * i0);
+    *reinterpret_cast<uint32_t*>(sQ + (row0 + g + 8) * kRow + col) = pack_half2(o[n][2] * i1, o[n][3] * i1);
+  }
+  __syncwarp();
+  const long obase = vid * batch_stride_o + pix * seq_stride_o + head * 64;
+  for (int i = lane; i < 16 * 8; i += 32) {
+    const int t = row0 + (i >> 3), piece = i & 7;
+    if (q0 + t < L)
+      *reinterpret_cast<uint4*>(out + obase + (long)(q0 + t) * tok_stride_o + piece * 8) =
+          *reinterpret_cast<const uint4*>(sQ + t * kRow + piece * 8);
+  }
+}
+
+// Generic small attention (any head_dim <= 64, any L), one thread per (seq, head, query): the frame transformers
+// with 4- or 8-channel heads (UNetSD_I2VGen's local temporal encoder, unet_i2vgen.py:122-124, and the VideoComposer
+// condition encoders, unet_videolcm.py:121-141; util.py:1396-1424), and head_dim 64 with unaligned operands.
 __global__ void attn_small_kernel(const __half* __restrict__ q, const __half* __restrict__ k, const __half* __restrict__ v,
                                   __half* __restrict__ out, long nseq, int heads, int L, int d, long tok_stride,
                                   long seq_stride, long tok_stride_o, long seq_stride_o, float scale, long spb,
@@ -262,7 +441,19 @@ extern "C" int vgen_attention_temporal(const void* q, const void* k, const void*
     VG_LAUNCH_CHECK("attn_temporal_kernel");
     return 0;
   }
-  VG_REQUIRE(head_dim <= 64 && L <= 64, "vgen_attention_temporal: unsupported (head_dim, L)");
+  if (head_dim == 64 && aligned) {
+    const long items = nseq * heads;
+    const long qtiles = (L + 63) / 64;
+    VG_REQUIRE(items <= 0x7fffffffL && qtiles <= 65535, "vgen_attention_temporal: too many sequences or frames");
+    const int warps = (int)((std::min<long>(L, 64) + 15) / 16);
+    const size_t smem = (size_t)(1 + 2 * (L > 64 ? 2 : 1)) * 64 * 72 * sizeof(__half);  // 27 KiB or 45 KiB
+    launch_kernel(attn_temporal_flash_kernel, dim3((unsigned)items, (unsigned)qtiles), dim3(32 * warps), smem, st, qp, kp, vp, op,
+                  (int)heads, (int)L, tok_stride, seq_stride, tok_stride_o, seq_stride_o, scale * 1.4426950408889634f, spb,
+                  batch_stride, batch_stride_o);
+    VG_LAUNCH_CHECK("attn_temporal_flash_kernel");
+    return 0;
+  }
+  VG_REQUIRE(head_dim <= 64, "vgen_attention_temporal: unsupported head_dim");
   const long total = nseq * heads * L;
   launch_kernel(attn_small_kernel, dim3((unsigned)((total + 127) / 128)), dim3(128), 0, st, qp, kp, vp, op, nseq, (int)heads, (int)L, (int)head_dim,
                                                                     tok_stride, seq_stride, tok_stride_o, seq_stride_o, scale, spb,

@@ -392,7 +392,7 @@ def attention_d512(q, k, v, out=None):
 
 def attention_temporal(q, k, v, heads, head_dim, out=None):
     """q/k/v [f, npix, heads*head_dim] views (frame-major) of one video, or [b, f, npix, heads*head_dim] for b videos back
-    to back (one launch): attention over the f tokens of each pixel."""
+    to back (one launch): attention over the f tokens of each pixel, for any f and any head_dim <= 64."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _chk16(t, nm)
         if t.dim() not in (3, 4) or t.stride(-1) != 1:
