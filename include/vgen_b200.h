@@ -152,7 +152,7 @@ int vgen_im2col(const void* x, void* out, int64_t nimg, int64_t h, int64_t w, in
 int vgen_upsample_nearest2x(const void* x, void* y, int64_t nimg, int64_t h, int64_t w, int64_t c, void* stream);
 /* dst[r][0:cols] = src[r][0:cols] with row strides (torch.cat along channels, unet_t2v.py:269) */
 int vgen_copy2d(const void* src, int64_t lds, void* dst, int64_t ldd, int64_t rows, int64_t cols, void* stream);
-/* op: 0 silu(a), 1 a+b, 2 gelu(a), 3 a*s, 4 a+s*b  (fp16, fp32 math) */
+/* op: 0 silu(a), 1 a+b, 2 gelu(a), 3 a*s, 4 a+s*b, 5 relu(a)  (fp16, fp32 math) */
 int vgen_eltwise(int op, const void* a, const void* b, void* y, int64_t n, float s, void* stream);
 /* out = [gelu](silu_in?(a) @ w^T + bias) [+ res] for small m or tiny k (time / fps / context MLPs
  * unet_t2v.py:93-104, ResBlock emb_layers util.py:857-863, TransformerV2 linears util.py:1396-1452) */
@@ -173,6 +173,23 @@ int vgen_adaptive_avgpool(const void* x, void* y, int64_t nimg, int64_t h, int64
  * single_sketch / local_image_embedding, unet_videolcm.py:295-372 (unet_tf2tv.py:292-369), applied at :598-703 (:594-699) */
 int vgen_cond_stem(const void* x, int x_is_f32, int64_t b, int64_t cin, int64_t f, int64_t h, int64_t w, const float* weight,
                    const float* bias, int64_t cout, void* y, int64_t oh, int64_t ow, void* stream);
+
+/* ---- DPT neck and head of the MiDaS v3 depth annotator (dpt.cu; tools/annotator/depth/__init__.py:162-293) ------- */
+/* Scatter half of a ConvTranspose2d with kernel == stride == s: g [nimg*hp*wp][ldg] fp16 is the vgen_linear product with
+ * the weight repacked to rows (ky, kx, co); out[b][y*s+ky][x*s+kx][co] = fp16(g[(b*hp+y)*wp+x][(ky*s+kx)*cout+co] +
+ * bias[co]), channels-last [nimg][s*hp][s*wp][cout].  cout, ldg multiples of 8; g / bias / out 16-byte aligned.
+ * replaces: nn.ConvTranspose2d(c, c, 4, stride=4) / (c, c, 2, stride=2), depth/__init__.py:202,212 */
+int vgen_dpt_tconv_scatter(const void* g, int64_t ldg, const float* bias, void* out, int64_t nimg, int64_t hp, int64_t wp,
+                           int64_t s, int64_t cout, void* stream);
+/* F.interpolate(scale_factor=2, mode='bilinear', align_corners=True) on [nimg][h][w][c] fp16 -> [nimg][2h][2w][c]
+ * (source coordinate dst * (in - 1) / (out - 1) in fp32, as PyTorch computes it); c a multiple of 8.
+ * replaces: depth/__init__.py:158 (FusionBlock), :238 (head nn.Upsample) */
+int vgen_upsample_bilinear2x_ac(const void* x, void* y, int64_t nimg, int64_t h, int64_t w, int64_t c, void* stream);
+/* Head tail: out[r] = relu(sum_k relu(x[r][k]) * w[k] + bias[0]) for rows r of x [rows][ldx] fp16 (the head's conv3x3
+ * output with its bias), w fp32 [c], bias fp32 [1] on the device; out fp16 or fp32 [rows] (= [n][1][H][W]).  c, ldx
+ * multiples of 8, c <= 1024.  replaces: ReLU -> nn.ConvTranspose2d(32, 1, 1) -> ReLU, depth/__init__.py:240-242 */
+int vgen_dpt_head_out(const void* x, int64_t ldx, int64_t rows, int64_t c, const float* w, const float* bias, void* out,
+                      int out_is_f32, void* stream);
 
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */

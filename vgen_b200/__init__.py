@@ -1,7 +1,8 @@
 """vgen_b200 -- H100-native (sm_90a) implementation of the VGen sampling hot path:
 DiffusionDDIM.ddim_sample_loop -> UNetSD_T2VBase / UNetSD_I2VGen (and the VideoLCM / TF-T2V / DreamVideo / InstructVideo
 LoRA / SR600 / HiGen variants, with the VideoComposer condition encoders and the DreamVideo adapters) forward ->
-AutoencoderKL.decode, exposed under the reference's MODEL / DIFFUSION / AUTO_ENCODER registry names (`register()`).
+AutoencoderKL.decode, exposed under the reference's MODEL / DIFFUSION / AUTO_ENCODER registry names (`register()`), and
+the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`).
 
 Every op of the path is a hand-written CUDA kernel in libvgen_b200.so (include/vgen_b200.h); this
 package holds only the host-side mirror of the reference interface.  There is no CPU / PyTorch
@@ -28,6 +29,9 @@ def __getattr__(name):  # lazy: importing the package must not require torch.cud
                 "FrozenOpenCLIPEmbedderZero"):
         from . import clip
         return getattr(clip, name)
+    if name in ("MiDaS", "midas_v3"):
+        from . import depth
+        return getattr(depth, name)
     if name == "LCMScheduler":
         from .lcm import LCMScheduler
         return LCMScheduler

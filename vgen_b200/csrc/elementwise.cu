@@ -127,7 +127,7 @@ __global__ void copy2d_kernel(const __half* __restrict__ src, long lds, __half* 
 }
 
 // ------------------------------------------------------------------ pointwise ops
-// op: 0 silu(a)  1 a+b  2 gelu(a) (erf)  3 a*s  4 a + s*b
+// op: 0 silu(a)  1 a+b  2 gelu(a) (erf)  3 a*s  4 a + s*b  5 relu(a)
 __global__ void eltwise_kernel(const __half* __restrict__ a, const __half* __restrict__ b, __half* __restrict__ y, long n,
                                int op, float s) {
   const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -139,7 +139,8 @@ __global__ void eltwise_kernel(const __half* __restrict__ a, const __half* __res
     case 1: r = x + __half2float(b[idx]); break;
     case 2: r = 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); break;
     case 3: r = x * s; break;
-    default: r = x + s * __half2float(b[idx]); break;
+    case 4: r = x + s * __half2float(b[idx]); break;
+    default: r = x < 0.f ? 0.f : x; break;  // NaN passes through, as in torch.relu
   }
   y[idx] = __float2half_rn(r);
 }
@@ -383,7 +384,7 @@ int vgen_copy2d(const void* src, int64_t lds, void* dst, int64_t ldd, int64_t ro
 }
 
 int vgen_eltwise(int op, const void* a, const void* b, void* y, int64_t n, float s, void* stream) {
-  VG_REQUIRE(a && y && op >= 0 && op <= 4, "vgen_eltwise: bad arguments");
+  VG_REQUIRE(a && y && op >= 0 && op <= 5, "vgen_eltwise: bad arguments");
   VG_REQUIRE(!(op == 1 || op == 4) || b, "vgen_eltwise: binary op needs b");
   if (n == 0) return 0;
   launch_kernel(eltwise_kernel, dim3(nblk(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 

@@ -82,6 +82,9 @@ _SIGNATURES = {
     "vgen_gauss_x0": [_vp, _vp, _vp, _f32, _f32, _f32, _i32, _vp, _i64, _i64, _vp],
     "vgen_video_to_rgb8": [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp],
     "vgen_lincomb_f32": [_vp, _i64, _vp, _f32, _vp, _f32, _vp, _f32, _vp, _f32, _vp],
+    "vgen_dpt_tconv_scatter": [_vp, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp],
+    "vgen_upsample_bilinear2x_ac": [_vp, _vp, _i64, _i64, _i64, _i64, _vp],
+    "vgen_dpt_head_out": [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp],
 }
 _RESTYPES = {"vgen_last_error": ctypes.c_char_p, "vgen_launch_count": ctypes.c_int64,
              "vgen_group_norm_workspace_bytes": ctypes.c_int64}

@@ -559,7 +559,7 @@ def concat_channels(a, b):
     return out
 
 
-_ELT = {"silu": 0, "add": 1, "gelu": 2, "scale": 3, "axpy": 4}
+_ELT = {"silu": 0, "add": 1, "gelu": 2, "scale": 3, "axpy": 4, "relu": 5}
 
 
 def eltwise(op, a, b=None, s=1.0, out=None):
@@ -570,6 +570,65 @@ def eltwise(op, a, b=None, s=1.0, out=None):
     _l.check(rc, "vgen_eltwise")
     return out
 
+
+
+def conv_transpose_stride(x, w, bias, s):
+    """nn.ConvTranspose2d(cin, cout, s, stride=s) on channels-last x [nimg, h, w, cin] fp16 -> [nimg, s*h, s*w, cout]:
+    one tap-GEMM against w [s*s*cout, cin] (rows (ky, kx, co), pack_conv_transpose_weight) and a scatter that adds the
+    fp32 bias [cout]."""
+    _chk16(x, "x")
+    if x.dim() != 4 or not x.is_contiguous():
+        raise _l.VgenError("conv_transpose_stride: x must be contiguous [nimg, h, w, cin]")
+    nimg, h, wd, cin = x.shape
+    cout = w.shape[0] // (s * s)
+    if w.shape[0] != s * s * cout or w.shape[1] != cin:
+        raise _l.VgenError(f"conv_transpose_stride: weight {tuple(w.shape)} does not match cin={cin}, stride {s}")
+    if bias.dtype != torch.float32 or not bias.is_contiguous() or bias.numel() != cout:
+        raise _l.VgenError(f"conv_transpose_stride: bias must be contiguous fp32 [{cout}]")
+    g = linear(x.view(nimg * h * wd, cin), w)
+    out = torch.empty(nimg, s * h, s * wd, cout, device=x.device, dtype=torch.float16)
+    rc = _run("dpt_tconv_scatter", 0.0, 4.0 * out.numel(),
+              lambda: _l.load().vgen_dpt_tconv_scatter(_p(g), g.stride(0), _p(bias), _p(out), nimg, h, wd, s, cout, _stream()))
+    _l.check(rc, "vgen_dpt_tconv_scatter")
+    return out
+
+
+def pack_conv_transpose_weight(w):
+    """ConvTranspose2d weight [cin, cout, s, s] -> [s*s*cout, cin] with row (ky*s + kx)*cout + co."""
+    cin, cout, kh, kw = w.shape
+    return w.detach().permute(2, 3, 1, 0).reshape(kh * kw * cout, cin)
+
+
+def upsample_bilinear2x(x):
+    """F.interpolate(scale_factor=2, mode='bilinear', align_corners=True) on channels-last x [nimg, h, w, c] fp16."""
+    _chk16(x, "x")
+    if x.dim() != 4 or not x.is_contiguous():
+        raise _l.VgenError("upsample_bilinear2x: x must be contiguous [nimg, h, w, c]")
+    nimg, h, w, c = x.shape
+    y = torch.empty(nimg, 2 * h, 2 * w, c, device=x.device, dtype=torch.float16)
+    rc = _run("upsample_bilinear", 0.0, 2.0 * (x.numel() + y.numel()),
+              lambda: _l.load().vgen_upsample_bilinear2x_ac(_p(x), _p(y), nimg, h, w, c, _stream()))
+    _l.check(rc, "vgen_upsample_bilinear2x_ac")
+    return y
+
+
+def dpt_head_out(x, w, bias, out_dtype=torch.float16):
+    """relu(relu(x) @ w + bias) per pixel of x [..., c] fp16 (c % 8 == 0), w fp32 [c], bias fp32 [1] -> x.shape[:-1] in
+    out_dtype (fp16 or fp32)."""
+    _chk16(x, "x")
+    x2, ldx = _rows_view(x, "x")
+    rows, c = x2.shape
+    for t, nm, n in ((w, "w", c), (bias, "bias", 1)):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n or t.device != x.device:
+            raise _l.VgenError(f"dpt_head_out: {nm} must be contiguous fp32 [{n}] on {x.device}")
+    if out_dtype not in (torch.float16, torch.float32):
+        raise _l.VgenError("dpt_head_out: out_dtype must be fp16 or fp32")
+    out = torch.empty(x.shape[:-1], device=x.device, dtype=out_dtype)
+    rc = _run("dpt_head_out", 2.0 * rows * c, 2.0 * rows * c + out.numel() * out.element_size(),
+              lambda: _l.load().vgen_dpt_head_out(_p(x2), ldx, rows, c, _p(w), _p(bias), _p(out),
+                                                  1 if out_dtype == torch.float32 else 0, _stream()))
+    _l.check(rc, "vgen_dpt_head_out")
+    return out
 
 def linear_small(a, w, bias=None, residual=None, silu_in=False, gelu_out=False, out=None):
     _chk16(a, "a"), _chk16(w, "w")
