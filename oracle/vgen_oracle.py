@@ -1,11 +1,16 @@
 """TEST INFRASTRUCTURE ONLY -- the oracle for the VGen sampling hot path.
 
 A plain-PyTorch (fp32 by default) restatement of what the reference computes on the path
-    DiffusionDDIM.ddim_sample_loop -> UNetSD_T2VBase / UNetSD_I2VGen (+ VideoLCM / SR600 / HiGen variants)
-    forward -> AutoencoderKL.decode,
+    DiffusionDDIM.ddim_sample_loop -> UNetSD_T2VBase / UNetSD_I2VGen (+ VideoLCM / TFT2V with VideoComposer conditions,
+    SR600, HiGen, DreamVideo and LoRA variants) forward -> AutoencoderKL.decode,
 written from the reference's arithmetic, not from its module tree: every function works directly on a
 reference-format state_dict (dict name -> tensor) and derives the block structure from the key names.
 Each function cites the reference lines it follows (paths relative to the reference root).
+
+Every UNet runs one trunk (_unet_trunk) inside one forward skeleton (_unet_forward); a family's public forward supplies
+only its embeddings, context tokens, concat channels and trunk options.  UNetSD_LoRA's pairs are applied by the shared
+attention at the scale the state-dict view carries (_SD.lora_scale); DreamVideo's adapters are an option of the shared
+transformer block (_Adapters).  Both are found from the state-dict keys.
 
 Pinning: the reference has no tests or golden vectors for this path (SURVEY.md section 4), so the
 oracle is pinned against the reference ITSELF, imported on CPU through oracle/refload.py:
@@ -19,6 +24,7 @@ this module.  The product (vgen_b200/) never does.
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass
 
 import torch
 import torch.nn.functional as F
@@ -138,13 +144,13 @@ def sinusoidal_embedding(t, dim):
 
 
 class _SD:
-    """state_dict view with a prefix."""
+    """state_dict view with a prefix.  lora_scale: the scale UNetSD_LoRA's pairs in sd are applied at (_proj)."""
 
-    def __init__(self, sd, prefix=""):
-        self.sd, self.p = sd, prefix
+    def __init__(self, sd, prefix="", lora_scale=1.0):
+        self.sd, self.p, self.lora_scale = sd, prefix, lora_scale
 
     def sub(self, name):
-        return _SD(self.sd, f"{self.p}{name}.")
+        return _SD(self.sd, f"{self.p}{name}.", self.lora_scale)
 
     def __getitem__(self, name):
         return self.sd[self.p + name]
@@ -168,10 +174,20 @@ def _lin(x, s):
     return F.linear(x, s["weight"], s.get("bias"))
 
 
+def _proj(x, s, name, lora):
+    """to_<name>(x), plus s.lora_scale * to_<name>_lora(x) when s holds that LoRA pair (unet_lora.py:114-131,161-195),
+    unmerged: x W^T (+ b) + s (x D^T) U^T."""
+    y = _lin(x, s.sub(name))
+    if s.has(lora + ".down_linear.weight"):
+        y = y + s.lora_scale * F.linear(F.linear(x, s[lora + ".down_linear.weight"]), s[lora + ".up_linear.weight"])
+    return y
+
+
 def _attention(x, ctx, s, heads):
-    """MemoryEfficientCrossAttention, util.py:231-269: softmax(q k^T / sqrt(d)) v per head."""
+    """MemoryEfficientCrossAttention, util.py:231-269: softmax(q k^T / sqrt(d)) v per head.  With UNetSD_LoRA's pairs in
+    s it is that class's attention (unet_lora.py:134-195), the pairs applied at s.lora_scale."""
     ctx = x if ctx is None else ctx
-    q, k, v = _lin(x, s.sub("to_q")), _lin(ctx, s.sub("to_k")), _lin(ctx, s.sub("to_v"))
+    q, k, v = _proj(x, s, "to_q", "to_q_lora"), _proj(ctx, s, "to_k", "to_k_lora"), _proj(ctx, s, "to_v", "to_v_lora")
     b, lq, inner = q.shape
     d = inner // heads
 
@@ -180,17 +196,51 @@ def _attention(x, ctx, s, heads):
 
     o = F.scaled_dot_product_attention(split(q), split(k), split(v))
     o = o.permute(0, 2, 1, 3).reshape(b, lq, inner)
-    return _lin(o, s.sub("to_out.0"))
+    return _proj(o, s, "to_out.0", "to_out_lora")
 
 
-def _basic_block(x, ctx, s, heads):
-    """BasicTransformerBlock.forward, util.py:700-704 (attn2 is self-attention when ctx is None);
-    FeedForward/GEGLU :707-741 (exact erf GELU)."""
-    x = _attention(_ln(x, s.sub("norm1")), None, s.sub("attn1"), heads) + x
-    x = _attention(_ln(x, s.sub("norm2")), ctx, s.sub("attn2"), heads) + x
-    h = _ln(x, s.sub("norm3"))
-    val, gate = _lin(h, s.sub("ff.net.0.proj")).chunk(2, dim=-1)
-    x = _lin(val * F.gelu(gate), s.sub("ff.net.2")) + x
+@dataclass(frozen=True)
+class _Adapters:
+    """UNetSD_DreamVideo's adapter arguments (unet_dreamvideo.py:225-290): the position ("serial" / "parallel") of the
+    adapter after each sublayer (attn1, attn2, ff) of the spatial and of the temporal transformers, the reference's
+    constructor defaults otherwise; the temporal adapters' condition [b, f, C] and ag_strength [b] (None without one).
+    Which sublayers carry an adapter is read from the state dict."""
+    spatial: tuple = ("", "parallel", "")
+    temporal: tuple = ("parallel", "parallel", "parallel")
+    cond: torch.Tensor | None = None
+    lam: torch.Tensor | None = None
+
+
+_NO_ADAPTERS = _Adapters()
+_ADAPTER_SITES = ("attn_adapter", "cross_attn_adapter", "ff_adapter")
+
+
+def _adapter(x, s, cond, lam):
+    """Adapter.forward, util.py:510-517 (lam broadcasts over the rows of x)."""
+    x_in = x
+    if cond is not None and s.has("condition_linear.weight"):
+        x = x + lam * _lin(cond, s.sub("condition_linear"))
+    return _lin(F.gelu(_lin(x, s.sub("down_linear"))), s.sub("up_linear")) + x_in
+
+
+def _basic_block(x, ctx, s, heads, disable_self_attn=False, positions=(), cond=None, lam=None):
+    """BasicTransformerBlock.forward, util.py:700-704 (attn2 is self-attention when ctx is None; with disable_self_attn
+    attn1 reads ctx too); FeedForward/GEGLU :707-741 (exact erf GELU).  Where s holds an adapter after a sublayer it is
+    BasicTransformerBlockWithAdapter.forward, util.py:649-672: positions[i] places the adapter of sublayer i, cond / lam
+    are the rows' condition and ag_strength."""
+    def ff(z):
+        val, gate = _lin(z, s.sub("ff.net.0.proj")).chunk(2, dim=-1)
+        return _lin(val * F.gelu(gate), s.sub("ff.net.2"))
+    subs = (lambda z: _attention(_ln(z, s.sub("norm1")), ctx if disable_self_attn else None, s.sub("attn1"), heads),
+            lambda z: _attention(_ln(z, s.sub("norm2")), ctx, s.sub("attn2"), heads),
+            lambda z: ff(_ln(z, s.sub("norm3"))))
+    for i, (site, sub) in enumerate(zip(_ADAPTER_SITES, subs)):
+        if not s.has(site + ".down_linear.weight"):
+            x = sub(x) + x
+        elif positions[i] == "parallel":
+            x = sub(x) + _adapter(x, s.sub(site), cond, lam)
+        else:
+            x = _adapter(sub(x) + x, s.sub(site), cond, lam)
     return x
 
 
@@ -222,26 +272,33 @@ def _res_block(x, emb, s, batch, woimg=False):
     return h5.permute(0, 2, 1, 3, 4).reshape(bf, c, hh, ww)
 
 
-def _spatial_transformer(x, ctx, s, head_dim):
-    """SpatialTransformer.forward (use_linear=True), util.py:354-373."""
+def _spatial_transformer(x, ctx, s, head_dim, adapters=_NO_ADAPTERS):
+    """SpatialTransformer.forward (use_linear=True), util.py:354-373; SpatialTransformerWithAdapter, util.py:603-648."""
     bf, c, hh, ww = x.shape
     h = _gn(x, s.sub("norm"), 1e-6).permute(0, 2, 3, 1).reshape(bf, hh * ww, c)
     h = _lin(h, s.sub("proj_in"))
-    h = _basic_block(h, ctx, s.sub("transformer_blocks.0"), h.shape[-1] // head_dim)
+    h = _basic_block(h, ctx, s.sub("transformer_blocks.0"), h.shape[-1] // head_dim, positions=adapters.spatial)
     h = _lin(h, s.sub("proj_out"))
     return h.reshape(bf, hh, ww, c).permute(0, 3, 1, 2) + x
 
 
-def _temporal_transformer(x, s, head_dim, batch, woimg=False):
+def _temporal_transformer(x, s, head_dim, batch, woimg=False, adapters=_NO_ADAPTERS):
     """TemporalTransformer.forward (use_linear=False, only_self_att=True), util.py:1240-1286.
-    x: [(b f), c, h, w]; tokens are the f frames of one pixel; both attentions are self-attention."""
+    x: [(b f), c, h, w]; tokens are the f frames of one pixel; both attentions are self-attention.
+    TemporalTransformerWithAdapter.forward, util.py:1340-1380: the adapters' condition [b, f, C] is broadcast over the pixels."""
     bf, c, hh, ww = x.shape
     f = bf // batch
     x5 = x.reshape(batch, f, c, hh, ww).permute(0, 2, 1, 3, 4)           # b c f h w
     h = F.group_norm(x5, 32, s["norm.weight"], s["norm.bias"], 1e-6)
     h = h.permute(0, 3, 4, 2, 1).reshape(batch * hh * ww, f, c)          # (b h w) f c
     h = F.linear(h, s["proj_in.weight"][:, :, 0], s["proj_in.bias"])     # Conv1d k=1 == per-token linear
-    h = _basic_block(h, None, s.sub("transformer_blocks.0"), h.shape[-1] // head_dim)
+    cond = lam = None
+    if adapters.cond is not None:
+        cd = adapters.cond.shape[-1]
+        cond = adapters.cond[:, None, None].expand(batch, hh, ww, f, cd).reshape(batch * hh * ww, f, cd)
+        lam = adapters.lam.repeat_interleave(hh * ww).view(-1, 1, 1)
+    h = _basic_block(h, None, s.sub("transformer_blocks.0"), h.shape[-1] // head_dim, positions=adapters.temporal,
+                     cond=cond, lam=lam)
     h = F.linear(h, s["proj_out.weight"][:, :, 0], s["proj_out.bias"])
     h = h.reshape(batch, hh, ww, f, c).permute(0, 3, 4, 1, 2).reshape(bf, c, hh, ww)
     if woimg and f == 1:                                                 # TemporalTransformerWoImg, unet_higen.py:146-149
@@ -249,15 +306,15 @@ def _temporal_transformer(x, s, head_dim, batch, woimg=False):
     return h + x
 
 
-def _run_block(x, s, emb, ctx, head_dim, batch, woimg=False, sr600=False):
+def _run_block(x, s, emb, ctx, head_dim, batch, woimg=False, sr600=False, adapters=_NO_ADAPTERS):
     """One entry of input_blocks / middle_block / output_blocks: dispatch on the parameters present
     (the reference dispatches on module type, unet_t2v.py:280-348)."""
     if s.has("in_layers.0.weight"):
         return _res_block(x, emb, s, batch, woimg)
     if s.has("transformer_blocks.0.norm1.weight"):
         if s["proj_in.weight"].ndim == 2:
-            return _spatial_transformer(x, ctx, s, head_dim)
-        return _temporal_transformer(x, s, head_dim, batch, woimg)
+            return _spatial_transformer(x, ctx, s, head_dim, adapters)
+        return _temporal_transformer(x, s, head_dim, batch, woimg, adapters)
     if s.has("op.weight"):                                    # Downsample: conv3x3 stride 2, util.py:946
         # UNetSD_SR600 pads the height by 2 (unet_sr600.py:151-153) so that odd heights survive the round trip
         return F.conv2d(x, s["op.weight"], s["op.bias"], stride=2, padding=(2, 1) if sr600 else 1)
@@ -293,24 +350,30 @@ def fourier_filter(x, threshold, scale):
     return torch.fft.ifftn(xf, dim=(-2, -1)).real.to(dtype)
 
 
-def _unet_trunk(sd, x, emb, ctx, head_dim, batch, woimg=False, conv_in_add=None, sr600=False):
+def _unet_trunk(sd, x, emb, ctx, head_dim, batch, woimg=False, conv_in_add=None, sr600=False, lora_scale=1.0,
+                adapters=_NO_ADAPTERS):
     """encoder / middle / decoder with skip concatenation, unet_t2v.py:257-277.
     conv_in_add: tensor added right after the first conv (HiGen img_embedding, unet_higen.py:544-547);
-    sr600: backbone scaling + Fourier-filtered skips on the first two decoder blocks (unet_sr600.py:269-285)."""
-    root = _SD(sd)
+    sr600: backbone scaling + Fourier-filtered skips on the first two decoder blocks (unet_sr600.py:269-285);
+    lora_scale: the scale of the LoRA pairs in sd (UNetSD_LoRA); adapters: DreamVideo's adapter arguments."""
+    root = _SD(sd, lora_scale=lora_scale)
+
+    def run(x, s):
+        return _run_block(x, s, emb, ctx, head_dim, batch, woimg, sr600, adapters)
+
     skips = []
     for i in _children(sd, "input_blocks."):
         blk = root.sub(f"input_blocks.{i}")
         if blk.has("op.weight"):
-            x = _run_block(x, blk, emb, ctx, head_dim, batch, woimg, sr600)
+            x = run(x, blk)
         else:
             for j in _children(sd, blk.p):
-                x = _run_block(x, blk.sub(str(j)), emb, ctx, head_dim, batch, woimg, sr600)
+                x = run(x, blk.sub(str(j)))
                 if i == 0 and j == 0 and conv_in_add is not None:
                     x = x + conv_in_add
         skips.append(x)
     for j in _children(sd, "middle_block."):
-        x = _run_block(x, root.sub(f"middle_block.{j}"), emb, ctx, head_dim, batch, woimg)
+        x = run(x, root.sub(f"middle_block.{j}"))
     for n, i in enumerate(_children(sd, "output_blocks.")):
         skip = skips.pop()
         if sr600 and n < 2:
@@ -320,7 +383,7 @@ def _unet_trunk(sd, x, emb, ctx, head_dim, batch, woimg=False, conv_in_add=None,
         x = torch.cat([x, skip], dim=1)
         blk = root.sub(f"output_blocks.{i}")
         for j in _children(sd, blk.p):
-            x = _run_block(x, blk.sub(str(j)), emb, ctx, head_dim, batch, woimg, sr600)
+            x = run(x, blk.sub(str(j)))
     x = F.conv2d(F.silu(_gn(x, root.sub("out.0"), 1e-5)), sd["out.2.weight"], sd["out.2.bias"], padding=1)
     return x
 
@@ -329,73 +392,95 @@ def _mlp(x, s):
     return _lin(F.silu(_lin(x, s.sub("0"))), s.sub("2"))
 
 
+def _unet_forward(sd, x, t, ctx, head_dim, fps=None, frame_emb=(), concat=None, **trunk):
+    """What every UNet's forward does around its trunk (unet_t2v.py:210-277).  x [b,c,f,h,w]; t [b]; ctx [b,L,C] the
+    context tokens.  The time embedding (plus the fps embedding when fps is given) is repeated per frame, then the
+    per-frame terms frame_emb [(b f), E] are added in turn; ctx is repeated per frame; the concat channels [b,*,f,h,w]
+    follow x's.  The trunk (trunk: _unet_trunk's options) runs in the (b f) layout; the result is [b,c_out,f,h,w]."""
+    b, c, f, h, w = x.shape
+    dim = sd["time_embed.0.weight"].shape[1]
+    root = _SD(sd)
+    emb = _mlp(sinusoidal_embedding(t, dim).to(x.dtype), root.sub("time_embed"))
+    if fps is not None:
+        emb = emb + _mlp(sinusoidal_embedding(fps, dim).to(x.dtype), root.sub("fps_embedding"))
+    emb = emb.repeat_interleave(f, dim=0)
+    for e in frame_emb:
+        emb = emb + e
+    if concat is not None:
+        x = torch.cat([x, concat], dim=1)
+    xx = x.permute(0, 2, 1, 3, 4).reshape(b * f, -1, h, w)
+    out = _unet_trunk(sd, xx, emb, ctx.repeat_interleave(f, dim=0), head_dim, b, **trunk)
+    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
+
+
 def unet_t2v_forward(sd, x, t, y, fps=None, head_dim=64, use_fps_condition=False):
     """UNetSD_T2VBase.forward, unet_t2v.py:210-277.  x [b,4,f,h,w]; t [b]; y [b,L,1024]."""
-    b, c, f, h, w = x.shape
-    dim = sd["time_embed.0.weight"].shape[1]
-    root = _SD(sd)
-    emb = _mlp(sinusoidal_embedding(t, dim).to(x.dtype), root.sub("time_embed"))
-    if use_fps_condition and fps is not None:
-        emb = emb + _mlp(sinusoidal_embedding(fps, dim).to(x.dtype), root.sub("fps_embedding"))
-    emb = emb.repeat_interleave(f, dim=0)
-    ctx = y.repeat_interleave(f, dim=0)
-    xx = x.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
-    out = _unet_trunk(sd, xx, emb, ctx, head_dim, b)
-    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
+    return _unet_forward(sd, x, t, y, head_dim, fps=fps if use_fps_condition else None)
 
 
-def unet_videolcm_forward(sd, x, t, y, fps=None, head_dim=64, use_fps_condition=False):
-    """UNetSD_VideoLCM.forward with video_compositions == ['text'] (configs/videolcm_t2v_infer.yaml:67),
-    unet_videolcm.py:541-760: `concat` stays all-zero (:598), pre_image is an empty Sequential (:409,705),
-    the context is y alone (:713-726)."""
+# VideoComposer conditions of UNetSD_VideoLCM / UNetSD_TFT2V: forward keyword -> (encoder prefix, frame-transformer
+# prefix, input channels), unet_videolcm.py:295-372; and the order the forward sums them in, :599-699
+ENCODERS = {
+    "depth": ("depth_embedding", "depth_embedding_after", 1),
+    "motion": ("motion_embedding", "motion_embedding_after", 2),
+    "canny": ("canny_embedding", "canny_embedding_after", 1),
+    "masked": ("masked_embedding", "mask_embedding_after", 4),
+    "sketch": ("sketch_embedding", "sketch_embedding_after", 1),
+    "single_sketch": ("single_sketch_embedding", "single_sketch_embedding_after", 1),
+    "local_image": ("local_image_embedding", "local_image_embedding_after", 3),
+}
+SUM_ORDER = ("depth", "local_image", "motion", "canny", "sketch", "single_sketch", "masked")
+
+
+def _encode_condition(v, sd, kw, b, oh, ow):
+    """<kw>_embedding -> <kw>_embedding_after, unet_videolcm.py:599-607 -> [b, cd, f, h, w]."""
+    enc, after, _ = ENCODERS[kw]
+    s = _SD(sd).sub(enc)
+    f = v.shape[2]
+    z = v.permute(0, 2, 1, 3, 4).reshape(b * f, v.shape[1], v.shape[3], v.shape[4])
+    z = F.silu(F.conv2d(z, s["0.weight"], s["0.bias"], padding=1))
+    z = F.adaptive_avg_pool2d(z, (oh, ow))
+    z = F.silu(F.conv2d(z, s["3.weight"], s["3.bias"], stride=2, padding=1))
+    z = F.conv2d(z, s["5.weight"], s["5.bias"], stride=2, padding=1)
+    cd, h, w = z.shape[1:]
+    tok = z.reshape(b, f, cd, h, w).permute(0, 3, 4, 1, 2).reshape(b * h * w, f, cd)
+    tok = _local_temporal_encoder(tok, _SD(sd).sub(after))
+    return tok.reshape(b, h, w, f, cd).permute(0, 4, 3, 1, 2)
+
+
+def unet_videolcm_forward(sd, x, t, y, fps=None, head_dim=64, use_fps_condition=False, image=None, resolution=None,
+                          **conds):
+    """UNetSD_VideoLCM / UNetSD_TFT2V.forward in eval(), unet_videolcm.py:541-784 (unet_tf2tv.py is the same forward).
+    conds: pixel-space conditions [b, ch, f, H, W] under ENCODERS' keywords, each encoded at resolution ([W, H]) / 2 and
+    summed into `concat` in the forward's order; image [b, 1, 1024]: its tokens follow y's in the context.
+    With y alone (video_compositions == ['text'], configs/videolcm_t2v_infer.yaml:67) `concat` stays all-zero (:598),
+    pre_image is an empty Sequential (:409,705) and the context is y (:713-726)."""
     b, c, f, h, w = x.shape
-    dim = sd["time_embed.0.weight"].shape[1]
-    root = _SD(sd)
-    concat_dim = sd["input_blocks.0.0.weight"].shape[1] - c
-    xx = torch.cat([x, x.new_zeros(b, concat_dim, f, h, w)], dim=1)
-    emb = _mlp(sinusoidal_embedding(t, dim).to(x.dtype), root.sub("time_embed"))
-    if use_fps_condition and fps is not None:
-        emb = emb + _mlp(sinusoidal_embedding(fps, dim).to(x.dtype), root.sub("fps_embedding"))
-    emb = emb.repeat_interleave(f, dim=0)
-    ctx = y.repeat_interleave(f, dim=0)
-    xx = xx.permute(0, 2, 1, 3, 4).reshape(b * f, c + concat_dim, h, w)
-    out = _unet_trunk(sd, xx, emb, ctx, head_dim, b)
-    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
+    concat = x.new_zeros(b, sd["input_blocks.0.0.weight"].shape[1] - c, f, h, w)
+    for kw in SUM_ORDER:
+        if conds.get(kw) is not None:
+            concat = concat + _encode_condition(conds[kw].to(x.dtype), sd, kw, b, resolution[1] // 2, resolution[0] // 2)
+    ctx = y
+    if image is not None:
+        ctx = torch.cat([ctx, _mlp(image, _SD(sd).sub("pre_image_condition")).view(b, -1, y.shape[-1])], dim=1)
+    return _unet_forward(sd, x, t, ctx, head_dim, fps=fps if use_fps_condition else None, concat=concat)
 
 
 def unet_sr600_forward(sd, x, t, y, head_dim=64):
     """UNetSD_SR600.forward, unet_sr600.py:220-299."""
-    b, c, f, h, w = x.shape
-    dim = sd["time_embed.0.weight"].shape[1]
-    emb = _mlp(sinusoidal_embedding(t, dim).to(x.dtype), _SD(sd).sub("time_embed")).repeat_interleave(f, dim=0)
-    ctx = y.repeat_interleave(f, dim=0)
-    xx = x.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
-    out = _unet_trunk(sd, xx, emb, ctx, head_dim, b, sr600=True)
-    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
-
-
-def _context_block_higen(x, ctx, s, heads):
-    """BasicTransformerBlock with disable_self_attn=True (util.py:700-704): attn1 is cross attention too."""
-    x = _attention(_ln(x, s.sub("norm1")), ctx, s.sub("attn1"), heads) + x
-    x = _attention(_ln(x, s.sub("norm2")), ctx, s.sub("attn2"), heads) + x
-    h = _ln(x, s.sub("norm3"))
-    val, gate = _lin(h, s.sub("ff.net.0.proj")).chunk(2, dim=-1)
-    return _lin(val * F.gelu(gate), s.sub("ff.net.2")) + x
+    return _unet_forward(sd, x, t, y, head_dim, sr600=True)
 
 
 def unet_higen_forward(sd, x, t, y, spat_prior, motion_cond, appearance_cond, fps=None, head_dim=64,
                        use_fps_condition=False):
     """UNetSD_HiGen.forward, unet_higen.py:401-467.
     embeddings (:436-443): per-frame time + motion (:387-396, linear interpolation of f-1 embeddings to f
-    frames) + appearance (:398-399); context (:444-445): TextContextCrossTransformerMultiLayer :154-172;
-    spat_prior enters through img_embedding right after the first conv (:544-547)."""
+    frames) + appearance (:398-399); context (:444-445): TextContextCrossTransformerMultiLayer :154-172, whose blocks
+    are BasicTransformerBlocks with disable_self_attn=True; spat_prior enters through img_embedding right after the
+    first conv (:544-547)."""
     b, c, f, h, w = x.shape
     dim = sd["time_embed.0.weight"].shape[1]
     root = _SD(sd)
-    emb = _mlp(sinusoidal_embedding(t, dim).to(x.dtype), root.sub("time_embed"))
-    if use_fps_condition and fps is not None:
-        emb = emb + _mlp(sinusoidal_embedding(fps, dim).to(x.dtype), root.sub("fps_embedding"))
-    emb = emb.repeat_interleave(f, dim=0)
     if f > 1:
         if motion_cond.size(1) != f:
             me = sinusoidal_embedding(motion_cond.flatten(0, 1), dim).view(b, f - 1, dim)
@@ -405,18 +490,15 @@ def unet_higen_forward(sd, x, t, y, spat_prior, motion_cond, appearance_cond, fp
         me = _mlp(me.to(x.dtype), root.sub("msim_embedding")).flatten(0, 1)
     else:
         me = _mlp(sinusoidal_embedding(motion_cond, dim).to(x.dtype), root.sub("msim_embedding"))
-    emb = emb + me
-    emb = emb + _mlp(appearance_cond.to(x.dtype), root.sub("asim_embedding")).flatten(0, 1)
+    ae = _mlp(appearance_cond.to(x.dtype), root.sub("asim_embedding")).flatten(0, 1)
     ce = root.sub("context_embedding")
     yy = _lin(y, ce.sub("input_mapping"))
     tok = sd["context_embedding.tokens"].to(x.dtype).repeat(b, 1, 1)
     for d in _children(sd, "context_embedding.context_transformer."):
-        tok = _context_block_higen(tok, yy, ce.sub(f"context_transformer.{d}"), 8)
-    ctx = _lin(tok, ce.sub("output_mapping")).repeat_interleave(f, dim=0)
+        tok = _basic_block(tok, yy, ce.sub(f"context_transformer.{d}"), 8, disable_self_attn=True)
     img = F.conv2d(spat_prior, sd["img_embedding.weight"], sd["img_embedding.bias"], padding=1).repeat_interleave(f, dim=0)
-    xx = x.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
-    out = _unet_trunk(sd, xx, emb, ctx, head_dim, b, woimg=True, conv_in_add=img)
-    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
+    return _unet_forward(sd, x, t, _lin(tok, ce.sub("output_mapping")), head_dim,
+                         fps=fps if use_fps_condition else None, frame_emb=(me, ae), woimg=True, conv_in_add=img)
 
 
 def _local_temporal_encoder(tok, s):
@@ -442,9 +524,8 @@ def _local_temporal_encoder(tok, s):
 
 
 def unet_i2vgen_forward(sd, x, t, y, image, local_image, fps, head_dim=64):
-    """UNetSD_I2VGen.forward, unet_i2vgen.py:243-346."""
+    """UNetSD_I2VGen.forward, unet_i2vgen.py:243-346; the embeddings (:298-299) are time + fps."""
     b, c, f, h, w = x.shape
-    dim = sd["time_embed.0.weight"].shape[1]
     root = _SD(sd)
     if local_image.ndim == 5 and local_image.size(2) > 1:
         local_image = local_image[:, :, :1]
@@ -466,10 +547,6 @@ def unet_i2vgen_forward(sd, x, t, y, image, local_image, fps, head_dim=64):
     tok = _local_temporal_encoder(tok, root.sub("local_temporal_encoder"))
     ximg = tok.reshape(b, h, w, f, cc).permute(0, 4, 3, 1, 2)
     concat = ximg + ximg  # "concat += _ximg" twice, :294-295 (acknowledged upstream bug, reproduced)
-    # [Embeddings] :298-299
-    emb = _mlp(sinusoidal_embedding(t, dim).to(x.dtype), root.sub("time_embed")) + \
-        _mlp(sinusoidal_embedding(fps, dim).to(x.dtype), root.sub("fps_embedding"))
-    emb = emb.repeat_interleave(f, dim=0)
     # [Context] :301-323 -- text tokens, 64 local-image tokens, num_tokens global-image tokens
     le = root.sub("local_image_embedding")
     li = local_image.permute(0, 2, 1, 3, 4).reshape(b, -1, h, w)
@@ -482,10 +559,27 @@ def unet_i2vgen_forward(sd, x, t, y, image, local_image, fps, head_dim=64):
     if image is not None:
         ce = _mlp(image, root.sub("context_embedding"))
         ctx = torch.cat([ctx, ce.view(b, -1, y.shape[-1])], dim=1)
-    ctx = ctx.repeat_interleave(f, dim=0)
-    xx = torch.cat([x, concat], dim=1).permute(0, 2, 1, 3, 4).reshape(b * f, -1, h, w)
-    out = _unet_trunk(sd, xx, emb, ctx, head_dim, b)
-    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
+    return _unet_forward(sd, x, t, ctx, head_dim, fps=fps, concat=concat)
+
+
+def unet_dreamvideo_forward(sd, ctor, x, t, y, y_image=None, ag_strength=None, head_dim=64):
+    """UNetSD_DreamVideo.forward in eval(), unet_dreamvideo.py:225-290; ctor: the reference's constructor kwargs (they
+    place the adapters).  y_image [b, 1 or f, C] conditions the temporal adapters at ag_strength, fp32 [b]: one per
+    video, where the reference takes one per batch (videos never interact, so a batch equals its videos run alone)."""
+    cond = lam = None
+    if y_image is not None and ctor.get("temporal_adapter_condition_dim"):
+        cond = y_image.repeat_interleave(x.shape[2], dim=1) if y_image.shape[1] == 1 else y_image
+        cond, lam = cond.to(x.dtype), ag_strength.to(x.device, x.dtype)
+    adapters = _Adapters(ctor.get("spatial_adapter_position_list", _NO_ADAPTERS.spatial),
+                         ctor.get("temporal_adapter_position_list", _NO_ADAPTERS.temporal), cond, lam)
+    return _unet_forward(sd, x, t, y, head_dim, adapters=adapters)
+
+
+def unet_lora_forward(sd, x, t, y, scale=1.0):
+    """UNetSD_LoRA.forward in eval() (unet_lora.py:1287-1344): UNetSD_T2VBase's forward, fps ignored, with the LoRA
+    pairs present in sd applied unmerged at `scale` (every adapted projection is x W^T + s (x D^T) U^T, two thin GEMMs
+    next to the base one, never the merged weight)."""
+    return _unet_forward(sd, x, t, y, head_dim=64, lora_scale=scale)
 
 
 # ------------------------------------------------------------------------------------ VAE decode

@@ -1,21 +1,21 @@
-"""InstructVideo (UNetSD_LoRA): parity cases, inputs and a plain-torch oracle of the unmerged LoRA UNet.
+"""InstructVideo (UNetSD_LoRA): parity cases, inputs and the oracle call.
 
-The oracle restates tools/modules/unet/unet_lora.py:134-195 (MemoryEfficientCrossAttention with its LoRA pairs) inside
-oracle/vgen_oracle.py's T2V trunk.  It never merges: every adapted projection is x W^T + s (x D^T) U^T, computed as two
-thin GEMMs next to the base one, so it cannot share the product's shortcut (the merge in the pack).
+The oracle of these cases is oracle/vgen_oracle.py's unet_lora_forward, which restates tools/modules/unet/unet_lora.py:134-195
+(MemoryEfficientCrossAttention with its LoRA pairs) in the shared T2V trunk.  It never merges: every adapted projection is
+x W^T + s (x D^T) U^T, computed as two thin GEMMs next to the base one, so it cannot share the product's shortcut (the merge
+in the pack).
 tools/make_golden_instructvideo.py freezes the reference's outputs for the cases and digests of its parameter lists
 (tests/golden/instructvideo_specs.json).
 """
 from __future__ import annotations
 
-import contextlib
 import json
 import os
 
 import torch
-import torch.nn.functional as F
 
-from oracle import synth, vgen_oracle as vo
+from oracle import synth
+from oracle.vgen_oracle import unet_lora_forward
 from oracle.cases import _FULL_UNET, _T2V_TINY, make_inputs as _base_inputs
 from _vcomp import spec_digest  # noqa: F401  (same digest format as vcomp_specs.json)
 
@@ -108,50 +108,6 @@ def load_spec(golden_dir, name, cases=None):
 def build_product(case):
     import vgen_b200
     return vgen_b200.UNetSD_LoRA(**case["ctor"])
-
-
-# ------------------------------------------------------------------------------------------------ oracle
-def _proj(x, s, name, lora, scale):
-    """to_<name>(x) + s * to_<name>_lora(x) (unet_lora.py:114-131,161-195), unmerged: x W^T (+ b) + s (x D^T) U^T."""
-    y = vo._lin(x, s.sub(name))
-    if s.has(lora + ".down_linear.weight"):
-        y = y + scale * F.linear(F.linear(x, s[lora + ".down_linear.weight"]), s[lora + ".up_linear.weight"])
-    return y
-
-
-def _attention_lora(scale):
-    def attention(x, ctx, s, heads):
-        ctx = x if ctx is None else ctx
-        q, k, v = _proj(x, s, "to_q", "to_q_lora", scale), _proj(ctx, s, "to_k", "to_k_lora", scale), \
-            _proj(ctx, s, "to_v", "to_v_lora", scale)
-        b, lq, inner = q.shape
-        d = inner // heads
-
-        def split(t):
-            return t.reshape(b, t.shape[1], heads, d).permute(0, 2, 1, 3)
-
-        o = F.scaled_dot_product_attention(split(q), split(k), split(v)).permute(0, 2, 1, 3).reshape(b, lq, inner)
-        return _proj(o, s, "to_out.0", "to_out_lora", scale)
-    return attention
-
-
-@contextlib.contextmanager
-def _lora_attention(scale):
-    """Runs vgen_oracle's trunk with every MemoryEfficientCrossAttention replaced by the LoRA one above (the blocks look
-    the attention up in the module at call time)."""
-    saved = vo._attention
-    vo._attention = _attention_lora(scale)
-    try:
-        yield
-    finally:
-        vo._attention = saved
-
-
-def unet_lora_forward(sd, x, t, y, scale=1.0):
-    """UNetSD_LoRA.forward in eval() (unet_lora.py:1287-1344): UNetSD_T2VBase's forward, fps ignored, with the LoRA
-    pairs present in sd applied unmerged at `scale`."""
-    with _lora_attention(scale):
-        return vo.unet_t2v_forward(sd, x, t, y)
 
 
 def oracle_call(case, sd, inp, y_key="y"):

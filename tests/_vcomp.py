@@ -1,7 +1,8 @@
-"""VideoComposer compositions of UNetSD_VideoLCM / UNetSD_TFT2V: parity cases, inputs and a plain-torch oracle.
+"""VideoComposer compositions of UNetSD_VideoLCM / UNetSD_TFT2V: parity cases, inputs and the oracle call.
 
-The oracle restates the reference's condition encoders and image tokens (tools/modules/unet/unet_videolcm.py:283-372,
-:598-745; unet_tf2tv.py is the same forward) on top of oracle/vgen_oracle.py's trunk.  tools/make_golden_vcomp.py
+The oracle of these cases is oracle/vgen_oracle.py's unet_videolcm_forward with the conditions, the image embedding and
+the resolution, which restates the reference's condition encoders and image tokens (tools/modules/unet/unet_videolcm.py:
+283-372, :598-745; unet_tf2tv.py is the same forward).  tools/make_golden_vcomp.py
 freezes the reference's own outputs for these cases into tests/golden/ (vcomp_*.npz, tft2v_tiny.npz, vcomp_pin.npz) and
 the reference's parameter lists as digests (vcomp_specs.json: tensor count, parameter count, sha256 of the list).
 """
@@ -12,25 +13,13 @@ import json
 import os
 
 import torch
-import torch.nn.functional as F
 
 from oracle import synth, vgen_oracle as vo
+from oracle.vgen_oracle import ENCODERS, SUM_ORDER
 from oracle.cases import CASES, FULL_CTORS, make_inputs as _base_inputs
 
 RELEASED = ["text", "mask", "depthmap", "sketch", "motion", "image", "local_image", "single_sketch"]
 EVERY = RELEASED + ["canny"]
-
-# forward keyword -> (encoder prefix, frame-transformer prefix, input channels), unet_videolcm.py:295-372
-ENCODERS = {
-    "depth": ("depth_embedding", "depth_embedding_after", 1),
-    "motion": ("motion_embedding", "motion_embedding_after", 2),
-    "canny": ("canny_embedding", "canny_embedding_after", 1),
-    "masked": ("masked_embedding", "mask_embedding_after", 4),
-    "sketch": ("sketch_embedding", "sketch_embedding_after", 1),
-    "single_sketch": ("single_sketch_embedding", "single_sketch_embedding_after", 1),
-    "local_image": ("local_image_embedding", "local_image_embedding_after", 3),
-}
-SUM_ORDER = ("depth", "local_image", "motion", "canny", "sketch", "single_sketch", "masked")   # :599-699
 
 _TINY = CASES["videolcm_tiny"]["ctor"]
 
@@ -120,50 +109,9 @@ def load_spec(golden_dir, name, cases=None):
     return spec
 
 
-def _encode(v, sd, kw, b, oh, ow):
-    """<kw>_embedding -> <kw>_embedding_after, unet_videolcm.py:599-607 -> [b, cd, f, h, w]."""
-    enc, after, _ = ENCODERS[kw]
-    s = vo._SD(sd).sub(enc)
-    f = v.shape[2]
-    z = v.permute(0, 2, 1, 3, 4).reshape(b * f, v.shape[1], v.shape[3], v.shape[4])
-    z = F.silu(F.conv2d(z, s["0.weight"], s["0.bias"], padding=1))
-    z = F.adaptive_avg_pool2d(z, (oh, ow))
-    z = F.silu(F.conv2d(z, s["3.weight"], s["3.bias"], stride=2, padding=1))
-    z = F.conv2d(z, s["5.weight"], s["5.bias"], stride=2, padding=1)
-    cd, h, w = z.shape[1:]
-    tok = z.reshape(b, f, cd, h, w).permute(0, 3, 4, 1, 2).reshape(b * h * w, f, cd)
-    tok = vo._local_temporal_encoder(tok, vo._SD(sd).sub(after))
-    return tok.reshape(b, h, w, f, cd).permute(0, 4, 3, 1, 2)
-
-
-def unet_vcomp_forward(sd, x, t, y, resolution, image=None, fps=None, head_dim=64, use_fps_condition=False, **conds):
-    """UNetSD_VideoLCM / UNetSD_TFT2V.forward in eval() (unet_videolcm.py:541-784): conditions summed into `concat`
-    in the forward's order, image tokens appended after the text tokens."""
-    b, c, f, h, w = x.shape
-    dim = sd["time_embed.0.weight"].shape[1]
-    root = vo._SD(sd)
-    concat_dim = sd["input_blocks.0.0.weight"].shape[1] - c
-    concat = x.new_zeros(b, concat_dim, f, h, w)
-    for kw in SUM_ORDER:
-        if conds.get(kw) is not None:
-            concat = concat + _encode(conds[kw].to(x.dtype), sd, kw, b, resolution[1] // 2, resolution[0] // 2)
-    xx = torch.cat([x, concat], dim=1)
-    emb = vo._mlp(vo.sinusoidal_embedding(t, dim).to(x.dtype), root.sub("time_embed"))
-    if use_fps_condition and fps is not None:
-        emb = emb + vo._mlp(vo.sinusoidal_embedding(fps, dim).to(x.dtype), root.sub("fps_embedding"))
-    emb = emb.repeat_interleave(f, dim=0)
-    ctx = y
-    if image is not None:
-        ctx = torch.cat([ctx, vo._mlp(image, root.sub("pre_image_condition")).view(b, -1, y.shape[-1])], dim=1)
-    ctx = ctx.repeat_interleave(f, dim=0)
-    xx = xx.permute(0, 2, 1, 3, 4).reshape(b * f, c + concat_dim, h, w)
-    out = vo._unet_trunk(sd, xx, emb, ctx, head_dim, b)
-    return out.reshape(b, f, -1, h, w).permute(0, 2, 1, 3, 4)
-
-
 def oracle_call(case, sd, inp):
     kw = call_kwargs(case, inp)
-    return unet_vcomp_forward(sd, inp["x"], inp["t"], kw.pop("y"), case["resolution"], **kw)
+    return vo.unet_videolcm_forward(sd, inp["x"], inp["t"], kw.pop("y"), resolution=case["resolution"], **kw)
 
 
 def build_product(case):
