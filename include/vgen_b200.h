@@ -85,6 +85,17 @@ int vgen_adapter_condition(const void* c, int64_t rows, int64_t k, int64_t ldc, 
 int vgen_conv2d_3x3(const void* x, int64_t nimg, int64_t h, int64_t w_, int64_t c, const void* w, int64_t n,
                     void* out, int64_t ldo, const vgen_epilogue* epi, void* stream);
 
+/* Convolution with an arbitrary list of 1..33 (dy, dx) tap offsets on x [nimg][h][w][c] fp16 (zero padding), w fp16
+ * [n][ntaps*c] (tap-major K), output grid = input grid.  Output pixel (b, y, x) is written at
+ * out + b*h*out_stride_y + y*out_stride_y + x*out_stride_x (element strides), so one output phase of a transposed conv
+ * writes its strided sub-grid directly (out_stride_y != w * out_stride_x needs relu = 1).  relu = 1: relu(acc + bias) in
+ * fp32, one rounding (bias only in epi).
+ * replaces: nn.ConvTranspose2d(c, c, 4, 2, 1) as four 2x2-tap phases and the stride-1 3x3 convs + ReLU of
+ *   tools/annotator/sketch/sketch_simplification.py:27-73; CDCM's conv2_1..conv2_4 summed as one 33-tap conv,
+ *   pidinet.py:481-488 */
+int vgen_conv2d_taps(const void* x, int64_t nimg, int64_t h, int64_t w_, int64_t c, int64_t ntaps, const int32_t* dy,
+                     const int32_t* dx, const void* w, int64_t n, void* out, int64_t out_stride_y, int64_t out_stride_x,
+                     const vgen_epilogue* epi, int relu, void* stream);
 /* temporal (3,1,1) conv, pad (1,0,0), on [f][hw][c] fp16 (one video); w is [n][3*c], k = kt*c + ci.
  * replaces: nn.Conv3d in TemporalConvBlock_v2 util.py:1662-1680 */
 int vgen_tconv3(const void* x, int64_t f, int64_t hw, int64_t c, const void* w, int64_t n, void* out,
@@ -190,6 +201,32 @@ int vgen_upsample_bilinear2x_ac(const void* x, void* y, int64_t nimg, int64_t h,
  * multiples of 8, c <= 1024.  replaces: ReLU -> nn.ConvTranspose2d(32, 1, 1) -> ReLU, depth/__init__.py:240-242 */
 int vgen_dpt_head_out(const void* x, int64_t ldx, int64_t rows, int64_t c, const float* w, const float* bias, void* out,
                       int out_is_f32, void* stream);
+
+/* ---- VideoComposer sketch annotators (sketch.cu; tools/annotator/sketch/pidinet.py, sketch_simplification.py) ------ */
+/* Depthwise k x k conv (k = 3 or 5, zero padding, no bias) + ReLU on x [nimg][h][w][c] fp16, c a multiple of 64, wgt fp32
+ * [k*k][c].  pool = 1: the conv runs on the 2x2 max-pool of x (floored, as nn.MaxPool2d(2)), which is also written to
+ * pooled [nimg][h/2][w/2][c]; out is [nimg][h'][w'][c] with (h', w') the conv's grid.
+ * replaces: PDCBlock_converted pool -> conv1 -> relu2, pidinet.py:546-550 */
+int vgen_dwconv_relu(const void* x, int64_t nimg, int64_t h, int64_t w, int64_t c, int64_t k, const float* wgt, int pool,
+                     void* pooled, void* out, void* stream);
+/* CSAM followed by MapReduce on x [nimg][h][w][c] fp16 (c a multiple of 8): t = w1 [4][c] . relu(x) + b1 [4] and
+ * s = wm [c] . x per pixel into the fp32 workspaces t_ws [nimg*h*w][4] and s_ws [nimg*h*w], then
+ * e = sigmoid(conv3x3(t; w2 [4][3][3])) * s + bm[0] -> fp32 e [nimg][h][w].  All weights fp32 on the device.
+ * replaces: CSAM + MapReduce, pidinet.py:458-464,499-500 */
+int vgen_csam_mapreduce(const void* x, int64_t nimg, int64_t h, int64_t w, int64_t c, const float* w1, const float* b1,
+                        const float* w2, const float* wm, const float* bm, float* t_ws, float* s_ws, float* e, void* stream);
+/* PiDiNet's output: bilinear resize (align_corners=False) of the four fp32 side maps e_i [nimg][hw[2i]][hw[2i+1]] to
+ * H x W, classifier cw [4] + bias cw[4], sigmoid -> out fp16 or fp32 [nimg][1][H][W].  hw is a host array.
+ * replaces: pidinet.py:687-704 */
+int vgen_pidinet_fuse(const float* e1, const float* e2, const float* e3, const float* e4, const int64_t* hw, int64_t nimg,
+                      int64_t H, int64_t W, const float* cw, void* out, int out_is_f32, void* stream);
+/* 3x3 conv (zero padding) to one channel + bias + sigmoid: x [nimg][h][w][c] fp16 (c a multiple of 8), wgt fp32 [9][c],
+ * bias fp32 [1] -> out fp16 or fp32 [nimg][1][h][w].  replaces: nn.Conv2d(24, 1, 3, 1, 1) + nn.Sigmoid(),
+ * sketch_simplification.py:72-73 */
+int vgen_conv3x3_to1_sigmoid(const void* x, int64_t nimg, int64_t h, int64_t w, int64_t c, const float* wgt, const float* bias,
+                             void* out, int out_is_f32, void* stream);
+/* y = fp16((x - mean) / std) for count elements of fp32 or fp16 x.  replaces: sketch_simplification.py:78 */
+int vgen_sketch_normalize(const void* x, int x_is_f32, int64_t count, float mean, float std_, void* y, void* stream);
 
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */

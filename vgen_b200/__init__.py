@@ -2,7 +2,8 @@
 DiffusionDDIM.ddim_sample_loop -> UNetSD_T2VBase / UNetSD_I2VGen (and the VideoLCM / TF-T2V / DreamVideo / InstructVideo
 LoRA / SR600 / HiGen variants, with the VideoComposer condition encoders and the DreamVideo adapters) forward ->
 AutoencoderKL.decode, exposed under the reference's MODEL / DIFFUSION / AUTO_ENCODER registry names (`register()`), and
-the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`).
+the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`) and sketch annotators (`PiDiNet` / `pidinet_bsd`,
+`SketchSimplification` / `sketch_simplification_gan`).
 
 Every op of the path is a hand-written CUDA kernel in libvgen_b200.so (include/vgen_b200.h); this
 package holds only the host-side mirror of the reference interface.  There is no CPU / PyTorch
@@ -32,6 +33,9 @@ def __getattr__(name):  # lazy: importing the package must not require torch.cud
     if name in ("MiDaS", "midas_v3"):
         from . import depth
         return getattr(depth, name)
+    if name in ("PiDiNet", "pidinet_bsd", "SketchSimplification", "sketch_simplification_gan"):
+        from . import sketch
+        return getattr(sketch, name)
     if name == "LCMScheduler":
         from .lcm import LCMScheduler
         return LCMScheduler

@@ -215,6 +215,50 @@ int vgen_conv2d_3x3(const void* x, int64_t nimg, int64_t h, int64_t w_, int64_t 
   return finish_and_launch(&t, epi, stream);
 }
 
+int vgen_conv2d_taps(const void* x, int64_t nimg, int64_t h, int64_t w_, int64_t c, int64_t ntaps, const int32_t* dy,
+                     const int32_t* dx, const void* w, int64_t n, void* out, int64_t out_stride_y, int64_t out_stride_x,
+                     const vgen_epilogue* epi, int relu, void* stream) {
+  VG_REQUIRE(x && w && out && dy && dx, "vgen_conv2d_taps: null pointer");
+  VG_REQUIRE(nimg >= 0 && h > 0 && w_ > 0 && c > 0 && n > 0, "vgen_conv2d_taps: bad shape");
+  VG_REQUIRE(ntaps >= 1 && ntaps <= kMaxTaps, "vgen_conv2d_taps: 1 to 33 taps");
+  VG_REQUIRE(out_stride_x >= n && out_stride_y >= out_stride_x * w_, "vgen_conv2d_taps: output strides overlap");
+  for (int i = 0; i < ntaps; ++i)
+    VG_REQUIRE(dy[i] >= -127 && dy[i] <= 127 && dx[i] >= -127 && dx[i] <= 127, "vgen_conv2d_taps: tap offsets must be in [-127, 127]");
+  if (nimg == 0) return 0;
+  TapGemmArgs t{};
+  t.a = reinterpret_cast<const __half*>(x);
+  t.w = reinterpret_cast<const __half*>(w);
+  t.a_stride1 = c;
+  t.a_stride2 = c * w_;
+  t.a_stride3 = c * w_ * h;
+  TapGemmShape& s = t.shape;
+  s.c = (int)c;
+  s.d1 = (int)w_;
+  s.d2 = (int)h;
+  s.d3 = (int)nimg;
+  pick_box(w_, h, &s.box1, &s.box2);
+  s.num_taps = (int)ntaps;
+  for (int i = 0; i < ntaps; ++i) {
+    s.tap1[i] = (int8_t)dx[i];
+    s.tap2[i] = (int8_t)dy[i];
+    s.tap3[i] = 0;
+  }
+  s.n = (int)n;
+  {
+    int rc = fill_epilogue(&t, out, out_stride_x, epi);
+    if (rc) return rc;
+  }
+  VG_REQUIRE(!t.epi.row_stats && !t.epi.geglu, "vgen_conv2d_taps: no folded LayerNorm or GEGLU");
+  VG_REQUIRE(!relu || (!t.epi.residual && !t.epi.group_bias), "vgen_conv2d_taps: the ReLU epilogue goes with bias only");
+  t.epi.relu = relu ? 1 : 0;
+  if (out_stride_y != out_stride_x * w_) {   // a strided sub-grid (the tile-store kernels serve it with the ReLU epilogue)
+    VG_REQUIRE(relu, "vgen_conv2d_taps: a strided output needs relu = 1");
+    t.epi.out_s2 = out_stride_y;
+    t.epi.out_s3 = out_stride_y * h;
+  }
+  return finish_and_launch(&t, epi, stream);
+}
+
 int vgen_tconv3_batch(const void* x, int64_t batch, int64_t f, int64_t hw, int64_t c, const void* w, int64_t n, void* out,
                       int64_t ldo, const vgen_epilogue* epi, void* stream) {
   VG_REQUIRE(x && w && out, "vgen_tconv3: null pointer");

@@ -5,7 +5,7 @@
 
 namespace vg {
 
-static constexpr int kMaxTaps = 9;
+static constexpr int kMaxTaps = 33;   // the 33 distinct taps of PiDiNet's CDCM (four dilated 3x3 convs summed)
 static constexpr int kMaxBnGelu = 224;   // widest N tile of the GELU / row-bias epilogue (BN = 256 spills registers)
 
 // Division by a launch-time constant as multiply-high + shift (exact for 0 <= x < 2^31).  The persistent
@@ -45,7 +45,8 @@ struct TapGemmShape {
   int box1, box2;   // output tile = box1 x box2 positions (<= 128) of one i3
   int t1, t2;       // tiles along d1 / d2
   int num_taps;
-  int tap1[kMaxTaps], tap2[kMaxTaps], tap3[kMaxTaps];  // coordinate offsets per tap
+  int8_t tap1[kMaxTaps], tap2[kMaxTaps], tap3[kMaxTaps];  // coordinate offsets per tap (bytes keep the kernel parameters
+                                                        // about as small as with nine int taps)
   int n;            // output channels (rows of W)
   int bn;           // N tile
   int nb;           // ceil(n / bn)
@@ -79,6 +80,9 @@ struct TapGemmEpilogue {
   long ld_row_bias;
   int rows_per_group;
   FastDiv f_rows_per_group;  // filled by the wgmma launcher
+  int relu;                  // out = relu(acc * alpha + bias) in fp32, one rounding (no residual / per-frame bias)
+  long out_s2, out_s3;       // 0: output rows are ldo apart; else element strides of the output along d2 / d3, with
+                             // ldo the stride along d1 (one phase of a transposed conv writes a strided sub-grid)
 };
 
 struct TapGemmArgs {

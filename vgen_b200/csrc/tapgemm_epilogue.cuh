@@ -49,6 +49,7 @@ struct EpiTile {
   int i3;            // outermost coordinate (frame) of the tile
   int i1_0, i2_0;    // origin of the tile along d1 / d2 (TMA store coordinates)
   long row[2];       // output rows of this thread
+  long ooff[2];      // element offsets of those rows in the output
   bool row_ok[2];    // those rows are inside the tensor
 };
 
@@ -71,7 +72,7 @@ __device__ __forceinline__ bool tapgemm_vec_ok(const TapGemmEpilogue& e, int out
 
 // host side: can the output be written with TMA tile stores?
 inline bool tapgemm_out_tma_ok(const TapGemmEpilogue& e) {
-  return (reinterpret_cast<uintptr_t>(e.out) & 15) == 0 && (e.ldo & 7) == 0;
+  return (reinterpret_cast<uintptr_t>(e.out) & 15) == 0 && (e.ldo & 7) == 0 && (e.out_s2 & 7) == 0 && (e.out_s3 & 7) == 0;
 }
 
 // ---- staging-tile protocol ---------------------------------------------------------------------------
@@ -107,8 +108,9 @@ __device__ __forceinline__ float round_h(float x) { return __half2float(__float2
 // rstd and shifted by (-mean * rstd) * col_sum[n]; such launches carry no residual / per-frame bias.
 // kGelu: adapter down projection (util.py:512-515): gelu_erf(acc + bias + row_bias[row / rows_per_group]) in fp32 and one
 // fp16 rounding at the store (the fp32 row bias carries the adapter's condition term); no residual / per-frame bias.
+// kRelu: relu(acc * alpha + bias) in fp32 and one fp16 rounding at the store; no residual / per-frame bias.
 // q2 = 2 * (lane % 4): this thread's column pair inside every 8-column group.
-template <int BN, bool kGeglu, bool kLn, bool kGelu>
+template <int BN, bool kGeglu, bool kLn, bool kGelu, bool kRelu = false>
 __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, const TapGemmEpilogue& e, const EpiTile& t,
                                                       EpiStore& st, bool vec_ok, int out_n, int q2, float (&acc)[BN / 2]) {
   float ln_scale[2] = {e.alpha, e.alpha}, ln_shift[2] = {0.f, 0.f};   // kLn: rstd (* alpha) and -mean * rstd of the rows
@@ -121,7 +123,7 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
         ln_shift[h] = rs.y * e.alpha;
       }
   }
-  __half* orow[2] = {e.out + t.row[0] * e.ldo, e.out + t.row[1] * e.ldo};
+  __half* orow[2] = {e.out + t.ooff[0], e.out + t.ooff[1]};
   if constexpr (!kGeglu) {
     const int n0 = t.nb_i * BN;
     const __half* grow = e.group_bias ? e.group_bias + (long)fd_div(e.f_group_bias_div, t.i3) * e.ld_group_bias : nullptr;
@@ -181,6 +183,10 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
             }
             f0 = gelu_erf(f0);
             f1 = gelu_erf(f1);
+          }
+          if (kRelu) {
+            f0 = fmaxf(f0, 0.f);
+            f1 = fmaxf(f1, 0.f);
           }
           if (have_g) {
             // reference: h (fp16 conv output) + emb_out (fp16) -> fp16  (util.py:909-919)

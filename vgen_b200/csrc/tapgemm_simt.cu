@@ -45,6 +45,7 @@ __global__ void tapgemm_simt_kernel(const __half* __restrict__ A, long st1, long
     if (e.row_stats) a = fmaf(ln_shift, e.col_sum[n], a);
     if (e.row_bias) a += e.row_bias[(row / e.rows_per_group) * e.ld_row_bias + n];
     if (e.gelu) a = gelu_erf_s(a);
+    if (e.relu) a = fmaxf(a, 0.f);
     if (e.group_bias) a = __half2float(__float2half_rn(a)) + __half2float(e.group_bias[(long)(i3 / e.group_bias_div) * e.ld_group_bias + n]);
     if (e.residual) a = __half2float(__float2half_rn(a)) + __half2float(e.residual[row * e.ldr + n]);
   } else {
@@ -64,7 +65,8 @@ __global__ void tapgemm_simt_kernel(const __half* __restrict__ A, long st1, long
     const float g16 = __half2float(__float2half_rn(g));
     a = v16 * __half2float(__float2half_rn(gelu_erf_s(g16)));
   }
-  e.out[row * e.ldo + n] = __float2half_rn(a);
+  const long ooff = e.out_s2 ? (long)i1 * e.ldo + (long)i2 * e.out_s2 + (long)i3 * e.out_s3 : row * e.ldo;
+  e.out[ooff + n] = __float2half_rn(a);
 }
 
 int tapgemm_simt_launch(const TapGemmArgs& a, cudaStream_t stream) {

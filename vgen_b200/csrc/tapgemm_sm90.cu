@@ -47,13 +47,13 @@ struct alignas(64) TapGemmKernelParams {
 };
 
 // kEpi: bit 0 = GEGLU epilogue, bit 1 = LayerNorm folded into the epilogue (TapGemmEpilogue.row_stats), bit 2 = GELU with the
-// fp32 row bias (TapGemmEpilogue.gelu); BN (the wgmma N and the accumulator count) is a template parameter as well, so every
-// register index of the epilogue is a constant.
+// fp32 row bias (TapGemmEpilogue.gelu), bit 3 = ReLU (TapGemmEpilogue.relu); BN (the wgmma N and the accumulator count) is a
+// template parameter as well, so every register index of the epilogue is a constant.
 template <int BN, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_constant__ TapGemmKernelParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atom (8 rows x 128 B).
-  constexpr bool kGeglu = (kEpi & 1) != 0, kLn = (kEpi & 2) != 0, kGelu = (kEpi & 4) != 0;
+  constexpr bool kGeglu = (kEpi & 1) != 0, kLn = (kEpi & 2) != 0, kGelu = (kEpi & 4) != 0, kRelu = (kEpi & 8) != 0;
   constexpr int kBBytes = BN * kBK * 2;                            // multiple of 1024 (BN % 32 == 0)
   constexpr int kStageBytes = kABytes + kBBytes;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -187,8 +187,10 @@ __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_
       const int i1 = t.i1_0 + r1[h], i2 = t.i2_0 + r2[h];
       t.row_ok[h] = (r0 + 8 * h < rows_in_tile) && (i1 < s.d1) && (i2 < s.d2);
       t.row[h] = ((long)t.i3 * s.d2 + i2) * s.d1 + i1;
+      // strided output (transposed-conv phases) exists only with the ReLU epilogue: the other kinds keep dense rows
+      t.ooff[h] = (kRelu && e.out_s2) ? (long)i1 * e.ldo + (long)i2 * e.out_s2 + (long)t.i3 * e.out_s3 : t.row[h] * e.ldo;
     }
-    tapgemm_epilogue_tile<BN, kGeglu, kLn, kGelu>(s, e, t, est, vec_ok, out_n, q2, acc);
+    tapgemm_epilogue_tile<BN, kGeglu, kLn, kGelu, kRelu>(s, e, t, est, vec_ok, out_n, q2, acc);
   }
   epi_stage_drain(est);
 }
@@ -200,6 +202,7 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
   if (attr_once.need()) {
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if constexpr (BN < 256)
       VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if constexpr (BN % 64 == 0) {
@@ -215,6 +218,7 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
   if constexpr (BN < 256) {   // the GELU epilogue spills at BN = 256: the launcher never picks it (kMaxBnGelu)
     if (kind == 4) launch_kernel(tapgemm_sm90_kernel<BN, 4>, dim3(grid), dim3(kThreads), smem, stream, p);
   }
+  if (kind == 8) launch_kernel(tapgemm_sm90_kernel<BN, 8>, dim3(grid), dim3(kThreads), smem, stream, p);
   if (kind == 2) launch_kernel(tapgemm_sm90_kernel<BN, 2>, dim3(grid), dim3(kThreads), smem, stream, p);
   if (kind == 0) launch_kernel(tapgemm_sm90_kernel<BN, 0>, dim3(grid), dim3(kThreads), smem, stream, p);
   VG_LAUNCH_CHECK("tapgemm_sm90_kernel");
@@ -236,6 +240,9 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   if (a.epi.gelu) VG_REQUIRE(s.bn <= kMaxBnGelu, "tapgemm_sm90: the GELU epilogue needs BN <= 224");
   if (a.epi.gelu) VG_REQUIRE(!a.epi.geglu && !a.epi.row_stats && !a.epi.residual && !a.epi.group_bias && s.num_taps == 1 &&
                              s.d2 == 1 && s.d3 == 1, "tapgemm: the GELU / row-bias epilogue goes with a plain linear");
+  if (a.epi.relu) VG_REQUIRE(!a.epi.geglu && !a.epi.row_stats && !a.epi.gelu && !a.epi.residual && !a.epi.group_bias,
+                             "tapgemm: the ReLU epilogue goes with bias only");
+  VG_REQUIRE(!a.epi.out_s2 || a.epi.relu, "tapgemm_sm90: a strided output goes with the ReLU epilogue");
 
   TapGemmKernelParams p;
   p.s = s;
@@ -263,7 +270,8 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   if (p.out_tma) {
     const uint64_t ld = (uint64_t)a.epi.ldo * 2;
     const uint64_t dims[4] = {(uint64_t)out_n, (uint64_t)s.d1, (uint64_t)s.d2, (uint64_t)s.d3};
-    const uint64_t strides[3] = {ld, ld * s.d1, ld * s.d1 * s.d2};
+    const uint64_t strides[3] = {ld, a.epi.out_s2 ? (uint64_t)a.epi.out_s2 * 2 : ld * s.d1,
+                                 a.epi.out_s2 ? (uint64_t)a.epi.out_s3 * 2 : ld * s.d1 * s.d2};
     const uint32_t box[4] = {32, (uint32_t)s.box1, (uint32_t)s.box2, 1};
     int rc = make_tmap_f16(&p.map_out, a.epi.out, 4, dims, strides, box, 64);
     if (rc) return rc;
@@ -277,7 +285,7 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   int grid = sm_count();
   if (grid > s.total_tiles) grid = s.total_tiles;
   if (grid < 1) return 0;
-  const int kind = (a.epi.geglu ? 1 : 0) | (a.epi.row_stats ? 2 : 0) | (a.epi.gelu ? 4 : 0);
+  const int kind = (a.epi.geglu ? 1 : 0) | (a.epi.row_stats ? 2 : 0) | (a.epi.gelu ? 4 : 0) | (a.epi.relu ? 8 : 0);
   switch (s.bn) {
     case 32: return launch_bn<32>(p, kind, grid, smem, stream);
     case 64: return launch_bn<64>(p, kind, grid, smem, stream);

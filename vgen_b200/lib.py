@@ -85,6 +85,12 @@ _SIGNATURES = {
     "vgen_dpt_tconv_scatter": [_vp, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp],
     "vgen_upsample_bilinear2x_ac": [_vp, _vp, _i64, _i64, _i64, _i64, _vp],
     "vgen_dpt_head_out": [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp],
+    "vgen_conv2d_taps": [_vp, _i64, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _EP, _i32, _vp],
+    "vgen_dwconv_relu": [_vp, _i64, _i64, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp],
+    "vgen_csam_mapreduce": [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "vgen_pidinet_fuse": [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i32, _vp],
+    "vgen_conv3x3_to1_sigmoid": [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp],
+    "vgen_sketch_normalize": [_vp, _i32, _i64, _f32, _f32, _vp, _vp],
 }
 _RESTYPES = {"vgen_last_error": ctypes.c_char_p, "vgen_launch_count": ctypes.c_int64,
              "vgen_group_norm_workspace_bytes": ctypes.c_int64}

@@ -806,3 +806,121 @@ def add_rows_f32_(x, add):
     rc = _l.load().vgen_add_rows_f32(_p(x), _p(add), x.shape[0], add.numel(), _stream())
     _l.check(rc, "vgen_add_rows_f32")
     return x
+
+
+# ------------------------------------------------------------------------------------------------
+# sketch annotators (sketch.cu, and the tap-GEMM's arbitrary-tap entry)
+def conv2d_taps(x, w, taps, bias=None, relu=False, out=None, out_stride_y=None, out_stride_x=None):
+    """out[b, y, x, :] = epi(sum_t x[b, y + dy_t, x + dx_t, :] @ w[:, t*c:(t+1)*c]^T) with zero padding, for channels-last
+    x [nimg, h, w, c] fp16 and taps [(dy, dx), ...] (1..33).  relu: relu(acc + bias) in fp32.  With out given, output
+    pixel (b, y, x) lands at element b*h*out_stride_y + y*out_stride_y + x*out_stride_x of out (a strided sub-grid, which
+    goes with relu=True)."""
+    _chk16(x, "x")
+    if x.dim() != 4 or not x.is_contiguous():
+        raise _l.VgenError("conv2d_taps: x must be contiguous [nimg, h, w, c]")
+    nimg, h, wd, c = x.shape
+    nt, n = len(taps), w.shape[0]
+    if w.shape[1] != nt * c:
+        raise _l.VgenError(f"conv2d_taps: weight {tuple(w.shape)} does not match {nt} taps x c={c}")
+    if out is None:
+        out = torch.empty(nimg, h, wd, n, device=x.device, dtype=torch.float16)
+        out_stride_y, out_stride_x = wd * n, n
+    e, keep = _epilogue(n, bias=bias)
+    dy = (ctypes.c_int32 * nt)(*[int(t[0]) for t in taps])
+    dx = (ctypes.c_int32 * nt)(*[int(t[1]) for t in taps])
+    rc = _run("conv_taps", 2.0 * nimg * h * wd * n * nt * c, 2.0 * (x.numel() + w.numel() + nimg * h * wd * n),
+              lambda: _l.load().vgen_conv2d_taps(_p(x), nimg, h, wd, c, nt, dy, dx, _p(w), n, _p(out), int(out_stride_y),
+                                                 int(out_stride_x), ctypes.byref(e), 1 if relu else 0, _stream()),
+              tag=f"taps{nt} c{c} n{n}")
+    _l.check(rc, "vgen_conv2d_taps")
+    return out
+
+
+def _chk32(t, name, n, dev):
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n or t.device != dev:
+        raise _l.VgenError(f"{name} must be contiguous fp32 [{n}] on {dev}")
+
+
+def dwconv_relu(x, w, k, pool=False):
+    """relu(depthwise k x k conv) of channels-last x [nimg, h, w, c] fp16 (c % 64 == 0), w fp32 [k*k, c]; with pool the
+    conv runs on the floored 2x2 max-pool of x.  -> (out, pooled or None)."""
+    _chk16(x, "x")
+    if x.dim() != 4 or not x.is_contiguous():
+        raise _l.VgenError("dwconv_relu: x must be contiguous [nimg, h, w, c]")
+    nimg, h, wd, c = x.shape
+    _chk32(w, "dwconv_relu: w", k * k * c, x.device)
+    ho, wo = (h // 2, wd // 2) if pool else (h, wd)
+    out = torch.empty(nimg, ho, wo, c, device=x.device, dtype=torch.float16)
+    pooled = torch.empty_like(out) if pool else None
+    rc = _run("dwconv", 2.0 * out.numel() * k * k, 2.0 * (x.numel() + out.numel() * (2 if pool else 1)),
+              lambda: _l.load().vgen_dwconv_relu(_p(x), nimg, h, wd, c, k, _p(w), 1 if pool else 0, _p(pooled), _p(out),
+                                                 _stream()))
+    _l.check(rc, "vgen_dwconv_relu")
+    return out, pooled
+
+
+def csam_mapreduce(x, w1, b1, w2, wm, bm):
+    """MapReduce(CSAM(x)) of channels-last x [nimg, h, w, c] fp16: w1 fp32 [4, c], b1 [4], w2 [4, 3, 3], wm [c], bm [1]
+    -> fp32 [nimg, h, w]."""
+    _chk16(x, "x")
+    if x.dim() != 4 or not x.is_contiguous():
+        raise _l.VgenError("csam_mapreduce: x must be contiguous [nimg, h, w, c]")
+    nimg, h, wd, c = x.shape
+    for t, nm, n in ((w1, "w1", 4 * c), (b1, "b1", 4), (w2, "w2", 36), (wm, "wm", c), (bm, "bm", 1)):
+        _chk32(t, f"csam_mapreduce: {nm}", n, x.device)
+    t_ws = torch.empty(nimg * h * wd, 4, device=x.device, dtype=torch.float32)
+    s_ws = torch.empty(nimg * h * wd, device=x.device, dtype=torch.float32)
+    e = torch.empty(nimg, h, wd, device=x.device, dtype=torch.float32)
+    rc = _run("csam", 12.0 * x.numel(), 2.0 * x.numel() + 40.0 * e.numel(),
+              lambda: _l.load().vgen_csam_mapreduce(_p(x), nimg, h, wd, c, _p(w1), _p(b1), _p(w2), _p(wm), _p(bm), _p(t_ws),
+                                                    _p(s_ws), _p(e), _stream()))
+    _l.check(rc, "vgen_csam_mapreduce")
+    return e
+
+
+def pidinet_fuse(es, cw, H, W, out_dtype=torch.float16):
+    """sigmoid(cw[:4] . bilinear_resize(es, (H, W)) + cw[4]) for four fp32 side maps [nimg, h_i, w_i] -> [nimg, 1, H, W]."""
+    nimg = es[0].shape[0]
+    for e in es:
+        if e.dtype != torch.float32 or e.dim() != 3 or not e.is_contiguous() or e.shape[0] != nimg or e.device != es[0].device:
+            raise _l.VgenError("pidinet_fuse: side maps must be contiguous fp32 [nimg, h, w] on one device")
+    _chk32(cw, "pidinet_fuse: cw", 5, es[0].device)
+    if out_dtype not in (torch.float16, torch.float32):
+        raise _l.VgenError("pidinet_fuse: out_dtype must be fp16 or fp32")
+    out = torch.empty(nimg, 1, H, W, device=es[0].device, dtype=out_dtype)
+    hw = (ctypes.c_int64 * 8)(*[int(d) for e in es for d in e.shape[1:]])
+    rc = _run("pidinet_fuse", 40.0 * out.numel(), 16.0 * out.numel() + out.numel() * out.element_size(),
+              lambda: _l.load().vgen_pidinet_fuse(_p(es[0]), _p(es[1]), _p(es[2]), _p(es[3]), hw, nimg, H, W, _p(cw), _p(out),
+                                                  1 if out_dtype == torch.float32 else 0, _stream()))
+    _l.check(rc, "vgen_pidinet_fuse")
+    return out
+
+
+def conv3x3_to1_sigmoid(x, w, bias, out_dtype=torch.float16):
+    """sigmoid(3x3 conv to one channel + bias) of channels-last x [nimg, h, w, c] fp16; w fp32 [9, c], bias fp32 [1]
+    -> [nimg, 1, h, w] in out_dtype."""
+    _chk16(x, "x")
+    if x.dim() != 4 or not x.is_contiguous():
+        raise _l.VgenError("conv3x3_to1_sigmoid: x must be contiguous [nimg, h, w, c]")
+    nimg, h, wd, c = x.shape
+    _chk32(w, "conv3x3_to1_sigmoid: w", 9 * c, x.device)
+    _chk32(bias, "conv3x3_to1_sigmoid: bias", 1, x.device)
+    if out_dtype not in (torch.float16, torch.float32):
+        raise _l.VgenError("conv3x3_to1_sigmoid: out_dtype must be fp16 or fp32")
+    out = torch.empty(nimg, 1, h, wd, device=x.device, dtype=out_dtype)
+    rc = _run("conv3x3_to1", 18.0 * x.numel(), 2.0 * x.numel() + out.numel() * out.element_size(),
+              lambda: _l.load().vgen_conv3x3_to1_sigmoid(_p(x), nimg, h, wd, c, _p(w), _p(bias), _p(out),
+                                                         1 if out_dtype == torch.float32 else 0, _stream()))
+    _l.check(rc, "vgen_conv3x3_to1_sigmoid")
+    return out
+
+
+def sketch_normalize(x, mean, std):
+    """fp16((x - mean) / std) of a contiguous fp32 / fp16 CUDA tensor, same shape."""
+    if not x.is_cuda or not x.is_contiguous() or x.dtype not in (torch.float32, torch.float16):
+        raise _l.VgenError("sketch_normalize: x must be a contiguous fp32 / fp16 CUDA tensor")
+    y = torch.empty(x.shape, device=x.device, dtype=torch.float16)
+    rc = _l.load().vgen_sketch_normalize(_p(x), 1 if x.dtype == torch.float32 else 0, x.numel(), float(mean), float(std),
+                                         _p(y), _stream())
+    _l.check(rc, "vgen_sketch_normalize")
+    return y
