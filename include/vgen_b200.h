@@ -246,6 +246,10 @@ int vgen_attention_cross_small(const void* q, const void* k, const void* v, void
  * out[r][:] = fp16(table[ids[r]][:] + pos[r % L][:]) -- token_embedding(text) + positional_embedding (:190-191) */
 int vgen_embed_tokens(const int64_t* ids, const float* table, const float* pos, void* out, int64_t nrows, int64_t L,
                       int64_t W, int64_t vocab, void* stream);
+/* The same gather with textual-inversion vectors (tools/modules/embedding_manager.py:76-116): an id >= vocab selects row
+ * id - vocab of extra [n_extra][W] fp32; the caller checks 0 <= id < vocab + n_extra (extra may be NULL iff n_extra == 0) */
+int vgen_embed_tokens_extra(const int64_t* ids, const float* table, int64_t vocab, const float* extra, int64_t n_extra,
+                            const float* pos, void* out, int64_t nrows, int64_t L, int64_t W, void* stream);
 /* x[b][i] = fp16(x[b][i] + add[i]), i < n: "x = x + self.positional_embedding" of the vision tower
  * (utils/reward/open_clip/transformer.py VisionTransformer.forward) */
 int vgen_add_rows_f32(void* x, const float* add, int64_t batch, int64_t n, void* stream);

@@ -3,7 +3,9 @@ DiffusionDDIM.ddim_sample_loop -> UNetSD_T2VBase / UNetSD_I2VGen (and the VideoL
 LoRA / SR600 / HiGen variants, with the VideoComposer condition encoders and the DreamVideo adapters) forward ->
 AutoencoderKL.decode, exposed under the reference's MODEL / DIFFUSION / AUTO_ENCODER registry names (`register()`), and
 the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`) and sketch annotators (`PiDiNet` / `pidinet_bsd`,
-`SketchSimplification` / `sketch_simplification_gan`).
+`SketchSimplification` / `sketch_simplification_gan`), and DreamVideo's textual-inversion text path
+(`FrozenOpenCLIPCustomEmbedder` + `EmbeddingManager`, EMBEDDER / EMBEDMANAGER) with DDIM inversion
+(`DiffusionDDIM.ddim_reverse_sample_loop`).
 
 Every op of the path is a hand-written CUDA kernel in libvgen_b200.so (include/vgen_b200.h); this
 package holds only the host-side mirror of the reference interface.  There is no CPU / PyTorch
@@ -27,9 +29,12 @@ def __getattr__(name):  # lazy: importing the package must not require torch.cud
         from . import diffusion_gauss
         return getattr(diffusion_gauss, name)
     if name in ("FrozenOpenCLIPEmbedder", "FrozenOpenCLIPVisualEmbedder", "FrozenOpenCLIPTextVisualEmbedder",
-                "FrozenOpenCLIPEmbedderZero"):
+                "FrozenOpenCLIPEmbedderZero", "FrozenOpenCLIPCustomEmbedder"):
         from . import clip
         return getattr(clip, name)
+    if name == "EmbeddingManager":
+        from .embedding_manager import EmbeddingManager
+        return EmbeddingManager
     if name in ("MiDaS", "midas_v3"):
         from . import depth
         return getattr(depth, name)

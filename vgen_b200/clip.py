@@ -1,5 +1,6 @@
 """H100-native CLIP conditioning (SURVEY.md section 8f-4): drop-ins for the reference's `FrozenOpenCLIPEmbedder`,
-`FrozenOpenCLIPVisualEmbedder` and `FrozenOpenCLIPTextVisualEmbedder` (tools/modules/clip_embedder.py:10-245), i.e. the
+`FrozenOpenCLIPVisualEmbedder`, `FrozenOpenCLIPTextVisualEmbedder` and `FrozenOpenCLIPCustomEmbedder`
+(tools/modules/clip_embedder.py:10-370; the last takes DreamVideo's textual-inversion manager), i.e. the
 ViT-H/14 text and image towers of open_clip's `CLIP` driven as those classes drive them:
 
   text   tokenize -> token + positional embedding -> the first (24 - layer_idx) causal pre-LN blocks -> ln_final
@@ -127,23 +128,37 @@ class ClipModel(SpecModule):
         return ops.linear(h, W[p + "proj.w"], bias=W[p + "proj.b"], residual=x2).view(b, L, w)
 
     # ---- towers ----------------------------------------------------------------------------------
+    def text_tokens(self, tokens, layer_idx=0, extra=None):
+        """tokens int64 [b, 77] (CUDA) -> ln_final(tokens after the first n - layer_idx blocks), fp16 [b, 77, W].
+        extra (fp32 [n_extra, W], CUDA): learned embeddings; an id >= vocab embeds row id - vocab of it (textual
+        inversion, see embedding_manager.py), and every id must then be below vocab + n_extra (checked here, before
+        the possibly graph-replayed forward)."""
+        if extra is None:
+            return self._text_tokens(tokens, layer_idx)
+        ops.check_token_ids(tokens, self.cfg["text_cfg"]["vocab_size"] + extra.shape[0])
+        return self._text_tokens(tokens, layer_idx, extra.contiguous())
+
     @graphed
     @torch.no_grad()
-    def text_tokens(self, tokens, layer_idx=0):
-        """tokens int64 [b, 77] (CUDA) -> ln_final(tokens after the first n - layer_idx blocks), fp16 [b, 77, W]."""
+    def _text_tokens(self, tokens, layer_idx=0, extra=None):
         W = self._packed or self._pack()
         t = self.cfg["text_cfg"]
-        x = ops.embed_tokens(tokens.contiguous(), W["tok"], W["pos"])
+        if extra is None:
+            x = ops.embed_tokens(tokens.contiguous(), W["tok"], W["pos"])
+        else:
+            x = ops.embed_tokens_extra(tokens.contiguous(), W["tok"], extra, W["pos"], check=False)
         for i in range(t["layers"] - int(layer_idx)):
             x = self._block(x, W, f"transformer.resblocks.{i}.", t["heads"], True)
         b, L, w = x.shape
         return ops.layer_norm(x.view(b * L, w), W["ln_final.g"], W["ln_final.b"]).view(b, L, w)
 
     @torch.no_grad()
-    def encode_text(self, tokens, layer_idx=0):
-        """-> (xt fp32 [b, E], x fp32 [b, 77, W]) like clip_embedder.py:204-212 (fp32 out: the reference's CLIP is fp32)."""
-        x = self.text_tokens(tokens, layer_idx)
-        eot = tokens.argmax(dim=-1)                                           # index math, as in the reference
+    def encode_text(self, tokens, layer_idx=0, extra=None, pool_tokens=None):
+        """-> (xt fp32 [b, E], x fp32 [b, 77, W]) like clip_embedder.py:204-212 (fp32 out: the reference's CLIP is fp32).
+        With textual inversion `tokens` are the gather ids and `extra` the learned rows (text_tokens), and the pooled
+        end-of-text position is taken from `pool_tokens`, the rewritten ids (clip_embedder.py:358)."""
+        x = self.text_tokens(tokens, layer_idx, extra)
+        eot = (tokens if pool_tokens is None else pool_tokens).argmax(dim=-1)  # index math, as in the reference
         pooled = x[torch.arange(x.shape[0], device=x.device), eot].contiguous()
         xt = ops.linear_small(pooled, self._packed["text_projection.w"])
         return xt.float(), x.float()
@@ -263,6 +278,57 @@ class FrozenOpenCLIPTextVisualEmbedder(_EmbedderBase):
         xi = self.model.encode_image(image.to(self._dev())) if image is not None else None
         xt, x = self.model.encode_text(tokenize(text).to(self._dev()), self.layer_idx)
         return xi, xt, x
+
+    def encode_image(self, image):
+        return self.model.encode_image(image)
+
+    def encode(self, text):
+        return self(text=text)
+
+
+OPENAI_DATASET_MEAN = (0.48145466, 0.4578275, 0.40821073)      # utils/reward/open_clip/constants.py
+OPENAI_DATASET_STD = (0.26862954, 0.26130258, 0.27577711)
+
+
+def white_image(image_size):
+    """open_clip's eval transform (resize, centre crop, normalise with the OpenAI mean / std) of an all-255 RGB image:
+    the resize and crop leave a constant image constant, so it is (1 - mean) / std per channel, [1, 3, S, S] fp32."""
+    mean = torch.tensor(OPENAI_DATASET_MEAN, dtype=torch.float32).view(3, 1, 1)
+    std = torch.tensor(OPENAI_DATASET_STD, dtype=torch.float32).view(3, 1, 1)
+    return ((torch.ones(3, image_size, image_size) - mean) / std).unsqueeze(0)
+
+
+class FrozenOpenCLIPCustomEmbedder(_EmbedderBase):
+    """clip_embedder.py:306-370 (DreamVideo's embedder): both towers, and text through an optional textual-inversion
+    `EmbeddingManager` (vgen_b200.embedding_manager).  forward(image, text, embedding_manager) -> (xi | None, xt, x).
+    The manager's substitution runs on the host over the ids (EmbeddingManager.plan); the learned vectors enter in
+    the token-gather kernel, and the pooled end-of-text position follows the rewritten ids like the reference's."""
+
+    @property
+    def white_image(self):
+        """The open_clip eval transform of a white image (the reference builds it at vit_resolution; the transform
+        resizes and crops to the tower's input size, clip_embedder.py:323-324)."""
+        return white_image(self.model.cfg["vision_cfg"]["image_size"])
+
+    def forward(self, image=None, text=None, embedding_manager=None):
+        xi = self.model.encode_image(image.to(self._dev())) if image is not None else None
+        xt, x = self.encode_with_transformer(tokenize(text), embedding_manager)
+        return xi, xt, x
+
+    def encode_with_transformer(self, tokens, embedding_manager=None):
+        """tokens int64 [b, 77] -> (xt fp32 [b, E], x fp32 [b, 77, W]) (clip_embedder.py:348-358)."""
+        dev = self._dev()
+        if embedding_manager is None:
+            return self.model.encode_text(tokens.to(dev), self.layer_idx)
+        from .embedding_manager import EmbeddingManager
+        if not isinstance(embedding_manager, EmbeddingManager):
+            raise TypeError(f"vgen_b200 FrozenOpenCLIPCustomEmbedder: embedding_manager must be a "
+                            f"vgen_b200.embedding_manager.EmbeddingManager, got {type(embedding_manager).__name__} "
+                            "(build it after vgen_b200.register())")
+        ids, gather, extra = embedding_manager.plan(tokens, self.model.cfg["text_cfg"]["vocab_size"])
+        if extra is None:
+            return self.model.encode_text(ids.to(dev), self.layer_idx)
+        return self.model.encode_text(gather.to(dev), self.layer_idx, extra=extra.to(dev), pool_tokens=ids.to(dev))
 
     def encode_image(self, image):
         return self.model.encode_image(image)

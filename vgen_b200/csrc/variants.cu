@@ -177,18 +177,23 @@ __global__ void scale_copy2d_kernel(const __half* __restrict__ src, long lds, __
 using namespace vg;
 
 // ------------------------------------------------------------------ CLIP embeddings (clip_embedder.py:190-191)
-// out[r][:] = fp16(table[ids[r]][:] + pos[r % L][:]): token_embedding(text) + positional_embedding, fp32 like the
-// reference, rounded once.  One thread per 4 channels.
+// out[r][:] = fp16(row(ids[r])[:] + pos[r % L][:]): token_embedding(text) + positional_embedding, fp32 like the
+// reference, rounded once.  row(id) = table[id] for id < vocab, else extra[id - vocab] (the learned textual-inversion
+// vectors the embedding manager writes over the token embedding, tools/modules/embedding_manager.py:76-116).  Without an
+// extra table an id is clamped to the vocabulary; with one the host has range-checked the ids.  One thread per 4 channels.
 __global__ void embed_tokens_kernel(const long long* __restrict__ ids, const float* __restrict__ table,
-                                    const float* __restrict__ pos, __half* __restrict__ out, long nrows, int L, int W, long vocab) {
+                                    const float* __restrict__ extra, const float* __restrict__ pos, __half* __restrict__ out,
+                                    long nrows, int L, int W, long vocab, long n_extra) {
   const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int w4 = W >> 2;
   if (idx >= nrows * w4) return;
   const long r = idx / w4;
   const int c = (int)(idx - r * w4) * 4;
   long id = ids[r];
-  id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
-  const float4 a = __ldg(reinterpret_cast<const float4*>(table + id * W + c));
+  const long n = vocab + n_extra;
+  id = id < 0 ? 0 : (id >= n ? n - 1 : id);
+  const float* row = id < vocab ? table + id * W : extra + (id - vocab) * W;
+  const float4 a = __ldg(reinterpret_cast<const float4*>(row + c));
   const float4 b = __ldg(reinterpret_cast<const float4*>(pos + (r % L) * W + c));
   uint2 o;
   o.x = pack_half2(a.x + b.x, a.y + b.y);
@@ -272,16 +277,25 @@ int vgen_scale_copy2d(const void* src, int64_t lds, void* dst, int64_t ldd, int6
   return 0;
 }
 
-int vgen_embed_tokens(const int64_t* ids, const float* table, const float* pos, void* out, int64_t nrows, int64_t L, int64_t W,
-                      int64_t vocab, void* stream) {
-  VG_REQUIRE(ids && table && pos && out && nrows >= 0 && L > 0 && W > 0 && W % 4 == 0 && vocab > 0, "vgen_embed_tokens: bad arguments");
-  VG_REQUIRE(((reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(pos)) & 15) == 0 &&
-                 (reinterpret_cast<uintptr_t>(out) & 7) == 0, "vgen_embed_tokens: table / pos must be 16-byte aligned");
+int vgen_embed_tokens_extra(const int64_t* ids, const float* table, int64_t vocab, const float* extra, int64_t n_extra,
+                            const float* pos, void* out, int64_t nrows, int64_t L, int64_t W, void* stream) {
+  VG_REQUIRE(ids && table && pos && out && nrows >= 0 && L > 0 && W > 0 && W % 4 == 0 && vocab > 0 && n_extra >= 0 &&
+                 (extra != nullptr) == (n_extra > 0),
+             "vgen_embed_tokens: bad arguments");
+  VG_REQUIRE(((reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(extra) | reinterpret_cast<uintptr_t>(pos)) &
+              15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0,
+             "vgen_embed_tokens: table / extra / pos must be 16-byte aligned");
   if (nrows == 0) return 0;
   launch_kernel(embed_tokens_kernel, dim3(nblk(nrows * (W / 4), 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                reinterpret_cast<const long long*>(ids), table, pos, reinterpret_cast<__half*>(out), nrows, (int)L, (int)W, vocab);
+                reinterpret_cast<const long long*>(ids), table, extra, pos, reinterpret_cast<__half*>(out), nrows, (int)L,
+                (int)W, vocab, n_extra);
   VG_LAUNCH_CHECK("embed_tokens_kernel");
   return 0;
+}
+
+int vgen_embed_tokens(const int64_t* ids, const float* table, const float* pos, void* out, int64_t nrows, int64_t L, int64_t W,
+                      int64_t vocab, void* stream) {
+  return vgen_embed_tokens_extra(ids, table, vocab, nullptr, 0, pos, out, nrows, L, W, stream);
 }
 
 int vgen_add_rows_f32(void* x, const float* add, int64_t batch, int64_t n, void* stream) {

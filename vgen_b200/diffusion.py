@@ -6,8 +6,8 @@ Host side (kept in fp64 torch / Python exactly like the reference, so it is bit-
   * beta schedules `cosine`, `linear_sd` (+ zero-terminal-SNR rescale)     schedules.py:5-21,62-63,72-79,143-165
   * cumulative-product tables                                             diffusion_ddim.py:46-78
   * the timestep list  (1 + arange(0, T, T // S)).clamp(0, T-1).flip(0)   diffusion_ddim.py:250
-Only the sampling entry points used by the inference engines are provided: ddim_sample_loop and ddim_sample for
-var_type fixed_small / mean_type v|eps.  The arithmetic of the reference's p_mean_variance (:147-206: two model calls,
+Only the sampling entry points used by the inference engines are provided: ddim_sample_loop and ddim_sample, and the
+DDIM inversion ddim_reverse_sample_loop / ddim_reverse_sample (DreamVideo), for var_type fixed_small / mean_type v|eps.  The arithmetic of the reference's p_mean_variance (:147-206: two model calls,
 CFG mix, v -> x0) has no method of its own here -- it lives inside the fused step kernel; the training losses and PLMS are
 out of scope and absent (calling them raises AttributeError, not a fallback).  DiffusionDDIMReward (InstructVideo) samples
 like DiffusionDDIM; its reward fine-tuning methods raise NotImplementedError.
@@ -203,6 +203,73 @@ class DiffusionDDIM(object):
                 raise NotImplementedError("vgen_b200 DiffusionDDIM: clamp / percentile / condition_fn are not supported")
             # the step index is known on the host: no device->host read of t inside the loop
             xt, _ = self._ddim_step(xt, int(step), t, model, model_kwargs, guide_scale, ddim_timesteps, eta)
+        return xt
+
+
+    # ---- DDIM inversion (diffusion_ddim.py:256-287) -------------------------------------------------------------
+    def ddim_reverse_steps(self, ddim_timesteps):
+        """The inversion's timestep list, arange(0, T, T // S) (:282): ascending, no +1 shift."""
+        T = self.num_timesteps
+        return torch.arange(0, T, T // ddim_timesteps)
+
+    def reverse_step_coefficients(self, step, ddim_timesteps):
+        """The seven fp32 scalars of one inversion step x_t -> x_{t+stride}, in vgen_ddim_step's slots: the x0 / eps
+        pair of the forward step and then sqrt(a_next), sqrt(1 - a_next) where a_next is the fp64 table
+        cat([alphas_cumprod, 0]) at clamp(t + stride, 0, T) cast to fp32 (_i(), :10-16), the square roots in fp32 (:275-279);
+        no noise term."""
+        T = self.num_timesteps
+        t = int(step)
+        f32 = torch.float32
+        a_next = torch.cat([self.alphas_cumprod, self.alphas_cumprod.new_zeros([1])])[min(max(t + T // ddim_timesteps, 0), T)]
+        a_next = a_next.to(f32)
+        coef = [self.sqrt_alphas_cumprod[t].to(f32), self.sqrt_one_minus_alphas_cumprod[t].to(f32),
+                self.sqrt_recip_alphas_cumprod[t].to(f32), self.sqrt_recipm1_alphas_cumprod[t].to(f32),
+                torch.sqrt(a_next), torch.sqrt(1 - a_next), 0.0]
+        return [float(c) for c in coef]
+
+    def _reverse_step(self, xt, step, t, model, model_kwargs, guide_scale, ddim_timesteps, want_x0=False):
+        if self.var_type != "fixed_small" or self.mean_type not in ("v", "eps"):
+            raise NotImplementedError("vgen_b200 DiffusionDDIM: only var_type fixed_small with mean_type v|eps")
+        ts = self._scale_timesteps(t)
+        if guide_scale is None:
+            y_out, u_out = model(xt, ts, **model_kwargs), None
+        else:
+            assert isinstance(model_kwargs, list) and len(model_kwargs) == 2
+            y_out, u_out = cfg_forward(model, xt, ts, model_kwargs)
+        coef = self.reverse_step_coefficients(step, ddim_timesteps)
+        y16 = y_out if y_out.dtype == torch.float16 else y_out.to(torch.float16)
+        u16 = None if u_out is None else (u_out if u_out.dtype == torch.float16 else u_out.to(torch.float16))
+        xt = xt if (xt.dtype == torch.float32 and xt.is_contiguous()) else xt.float().contiguous()
+        xt = xt.clone()
+        x0 = torch.empty_like(xt) if want_x0 else None
+        ops.ddim_step_(xt, y16.contiguous(), None if u16 is None else u16.contiguous(), coef, guide_scale,
+                       mean_type_v=(self.mean_type == "v"), noise=None, x0_out=x0)
+        return xt, x0
+
+    @torch.no_grad()
+    def ddim_reverse_sample(self, xt, t, model, model_kwargs={}, clamp=None, percentile=None, guide_scale=None,
+                            ddim_timesteps=20):
+        """One deterministic inversion step x_t -> x_{t+stride} (diffusion_ddim.py:256-274): the forward step's x0 and
+        eps, then mu = sqrt(a_next) x0 + sqrt(1 - a_next) eps in the fused step kernel.  Returns (mu, x0).  All batch
+        entries share the timestep; no random numbers are drawn (nor does the reference draw any)."""
+        if clamp is not None or percentile is not None:
+            raise NotImplementedError("vgen_b200 DiffusionDDIM: clamp / percentile are not used by the supported "
+                                      "inference configs")
+        return self._reverse_step(xt, int(t.flatten()[0]), t, model, model_kwargs, guide_scale, ddim_timesteps,
+                                  want_x0=True)
+
+    @torch.no_grad()
+    def ddim_reverse_sample_loop(self, x0, model, model_kwargs={}, clamp=None, percentile=None, guide_scale=None,
+                                 ddim_timesteps=20):
+        """diffusion_ddim.py:276-287: DDIM inversion of x0 over arange(0, T, T // S) (DreamVideo's inverse_noise_strength,
+        inference_dreamvideo_entrance.py:199-209)."""
+        if clamp is not None or percentile is not None:
+            raise NotImplementedError("vgen_b200 DiffusionDDIM: clamp / percentile are not supported")
+        b = x0.size(0)
+        xt = x0
+        for step in self.ddim_reverse_steps(ddim_timesteps).tolist():
+            t = torch.full((b,), step, dtype=torch.long, device=xt.device)
+            xt, _ = self._reverse_step(xt, step, t, model, model_kwargs, guide_scale, ddim_timesteps)
         return xt
 
 

@@ -61,6 +61,7 @@ _SIGNATURES = {
     "vgen_softmax_rows": [_vp, _i64, _i64, _i64, _f32, _vp],
     "vgen_attention_cross_small": [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _f32, _vp],
     "vgen_embed_tokens": [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp],
+    "vgen_embed_tokens_extra": [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp],
     "vgen_add_rows_f32": [_vp, _vp, _i64, _i64, _vp],
     "vgen_interp_linear_rows": [_vp, _vp, _i64, _i64, _i64, _i64, _vp],
     "vgen_fourier_lowfreq_filter": [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _i64, _f32, _vp],

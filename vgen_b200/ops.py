@@ -798,6 +798,38 @@ def embed_tokens(ids, table, pos):
     return out
 
 
+def check_token_ids(ids, n_rows):
+    """Raise unless every id is in [0, n_rows): one small device-to-host read of (min, max)."""
+    if ids.numel():
+        lo, hi = (int(v) for v in torch.aminmax(ids))
+        if lo < 0 or hi >= n_rows:
+            raise _l.VgenError(f"embed_tokens: token ids span [{lo}, {hi}], outside the {n_rows} rows of the vocabulary "
+                               "plus the learned embeddings")
+
+
+def embed_tokens_extra(ids, table, extra, pos, check=True):
+    """embed_tokens with learned rows: an id >= vocab reads extra[id - vocab] (fp32 [n_extra, W]; None = no extra rows).
+    An id outside [0, vocab + n_extra) is an error, not a clamp: the ids are checked on the host before the launch.
+    check=False is for a caller that has already checked them (CUDA-graph capture cannot read them back)."""
+    if ids.dtype != torch.int64 or not ids.is_cuda or not ids.is_contiguous() or ids.dim() != 2:
+        raise _l.VgenError("embed_tokens: ids must be a contiguous CUDA int64 tensor [b, L]")
+    for t, nm in ((table, "table"), (pos, "pos")) + (() if extra is None else ((extra, "extra"),)):
+        if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+            raise _l.VgenError(f"embed_tokens: {nm} must be a contiguous CUDA fp32 tensor")
+    b, L = ids.shape
+    vocab, W = table.shape
+    n_extra = 0 if extra is None else extra.shape[0]
+    if pos.shape != (L, W) or (extra is not None and (extra.dim() != 2 or extra.shape[1] != W)):
+        raise _l.VgenError("embed_tokens: pos must be [L, W] and extra [n_extra, W]")
+    if check:
+        check_token_ids(ids, vocab + n_extra)
+    out = torch.empty(b, L, W, device=ids.device, dtype=torch.float16)
+    rc = _l.load().vgen_embed_tokens_extra(_p(ids), _p(table), vocab, _p(extra), n_extra, _p(pos), _p(out), b * L, L, W,
+                                           _stream())
+    _l.check(rc, "vgen_embed_tokens_extra")
+    return out
+
+
 def add_rows_f32_(x, add):
     """x fp16 [b, ...] += add fp32 [...] broadcast over the leading dim, in place."""
     _chk16(x, "x")

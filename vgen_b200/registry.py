@@ -53,25 +53,27 @@ class Registry:
         return _register
 
 
-MODEL = DIFFUSION = AUTO_ENCODER = EMBEDDER = None
+MODEL = DIFFUSION = AUTO_ENCODER = EMBEDDER = EMBEDMANAGER = None
 USING_REFERENCE_REGISTRY = False
 
 
 def register(force_local: bool = False):
     """Register the UNets (T2VBase, I2VGen, VideoLCM, TFT2V, DreamVideo, LoRA, SR600, HiGen), DiffusionDDIM(SR / Reward),
-    AutoencoderKL and the four FrozenOpenCLIP*Embedder classes under the reference's registry names.  Returns (MODEL,
-    DIFFUSION, AUTO_ENCODER); the embedder registry is `vgen_b200.registry.EMBEDDER`."""
-    global MODEL, DIFFUSION, AUTO_ENCODER, EMBEDDER, USING_REFERENCE_REGISTRY
+    AutoencoderKL, the five FrozenOpenCLIP*Embedder classes and DreamVideo's EmbeddingManager under the reference's
+    registry names.  Returns (MODEL, DIFFUSION, AUTO_ENCODER); the embedder and embedding-manager registries are
+    `vgen_b200.registry.EMBEDDER` and `vgen_b200.registry.EMBEDMANAGER`."""
+    global MODEL, DIFFUSION, AUTO_ENCODER, EMBEDDER, EMBEDMANAGER, USING_REFERENCE_REGISTRY
     from .autoencoder import AutoencoderKL
-    from .clip import (FrozenOpenCLIPEmbedder, FrozenOpenCLIPEmbedderZero, FrozenOpenCLIPTextVisualEmbedder,
-                       FrozenOpenCLIPVisualEmbedder)
+    from .clip import (FrozenOpenCLIPCustomEmbedder, FrozenOpenCLIPEmbedder, FrozenOpenCLIPEmbedderZero,
+                       FrozenOpenCLIPTextVisualEmbedder, FrozenOpenCLIPVisualEmbedder)
     from .diffusion import DiffusionDDIM, DiffusionDDIMReward
     from .diffusion_gauss import DiffusionDDIMSR
+    from .embedding_manager import EmbeddingManager
     from .unet import (UNetSD_DreamVideo, UNetSD_HiGen, UNetSD_I2VGen, UNetSD_LoRA, UNetSD_SR600, UNetSD_T2VBase,
                        UNetSD_TFT2V, UNetSD_VideoLCM)
 
     regs = None
-    emb = None
+    emb = emm = None
     if not force_local:
         try:
             from utils.registry_class import AUTO_ENCODER as A, DIFFUSION as D, MODEL as M  # the reference's singletons
@@ -84,6 +86,10 @@ def register(force_local: bool = False):
                 from utils.registry_class import EMBEDDER as emb  # noqa: N811
             except ImportError:   # an older reference tree without the embedder registry: keep the three above
                 emb = None
+            try:
+                from utils.registry_class import EMBEDMANAGER as emm  # noqa: N811
+            except ImportError:   # likewise for the embedding-manager registry (DreamVideo)
+                emm = None
     if regs is None:
         regs = (MODEL or Registry("MODEL"), DIFFUSION or Registry("DIFFUSION"), AUTO_ENCODER or Registry("AUTO_ENCODER"))
         USING_REFERENCE_REGISTRY = False
@@ -101,6 +107,8 @@ def register(force_local: bool = False):
         AUTO_ENCODER.register_class()(AutoencoderKL)
         EMBEDDER = emb if emb is not None else (EMBEDDER or Registry("EMBEDDER"))   # also reachable as vgen_b200.registry.EMBEDDER
         for cls in (FrozenOpenCLIPEmbedder, FrozenOpenCLIPVisualEmbedder, FrozenOpenCLIPTextVisualEmbedder,
-                    FrozenOpenCLIPEmbedderZero):
+                    FrozenOpenCLIPEmbedderZero, FrozenOpenCLIPCustomEmbedder):
             EMBEDDER.register_class()(cls)
+        EMBEDMANAGER = emm if emm is not None else (EMBEDMANAGER or Registry("EMBEDMANAGER"))
+        EMBEDMANAGER.register_class()(EmbeddingManager)
     return MODEL, DIFFUSION, AUTO_ENCODER
