@@ -163,7 +163,8 @@ int vgen_im2col(const void* x, void* out, int64_t nimg, int64_t h, int64_t w, in
 int vgen_upsample_nearest2x(const void* x, void* y, int64_t nimg, int64_t h, int64_t w, int64_t c, void* stream);
 /* dst[r][0:cols] = src[r][0:cols] with row strides (torch.cat along channels, unet_t2v.py:269) */
 int vgen_copy2d(const void* src, int64_t lds, void* dst, int64_t ldd, int64_t rows, int64_t cols, void* stream);
-/* op: 0 silu(a), 1 a+b, 2 gelu(a), 3 a*s, 4 a+s*b, 5 relu(a)  (fp16, fp32 math) */
+/* op: 0 silu(a), 1 a+b, 2 gelu(a), 3 a*s, 4 a+s*b, 5 relu(a), 6 quick_gelu(a) = a*sigmoid(1.702a)  (fp16, fp32 math;
+ * 6 is OpenAI CLIP's activation, open_clip transformer.py QuickGELU) */
 int vgen_eltwise(int op, const void* a, const void* b, void* y, int64_t n, float s, void* stream);
 /* out = [gelu](silu_in?(a) @ w^T + bias) [+ res] for small m or tiny k (time / fps / context MLPs
  * unet_t2v.py:93-104, ResBlock emb_layers util.py:857-863, TransformerV2 linears util.py:1396-1452) */
@@ -227,6 +228,27 @@ int vgen_conv3x3_to1_sigmoid(const void* x, int64_t nimg, int64_t h, int64_t w, 
                              void* out, int out_is_f32, void* stream);
 /* y = fp16((x - mean) / std) for count elements of fp32 or fp16 x.  replaces: sketch_simplification.py:78 */
 int vgen_sketch_normalize(const void* x, int x_is_f32, int64_t count, float mean, float std_, void* y, void* stream);
+
+/* ---- DreamVideo's evaluation metric (metric.cu; metric/cal_metric_DreamVideo.py) ------------------------------------ */
+/* torchvision Resize(short side, BICUBIC) -> CenterCrop -> ToTensor -> Normalize of n uint8 RGB images src [n][h][w][3],
+ * bit-exact with Pillow's 8-bit ImagingResample (libImaging/Resample.c).  The host passes Pillow's fixed-point tables
+ * (22 fractional bits) for the crop's columns and rows only: hbounds [cw][2] = (first source column, taps) and hcoef
+ * [cw][kh]; vbounds [ch][2] = (first source row, taps) and vcoef [ch][kv] (an axis Pillow leaves alone: one tap of
+ * 1 << 22).  tile_rows is the largest number of source rows the vertical windows of 16 consecutive output rows span.
+ * out: fp16 channels-last [n][ch][cw][3] (out_f32 = 0, the towers' input) or fp32 [n][3][ch][cw] (out_f32 = 1, what
+ * torchvision returns); (u / 255 - mean[c]) / std[c] in IEEE fp32.
+ * replaces: clip_preprocess / dino_preprocess (with T.ToPILImage) per frame, cal_metric_DreamVideo.py:70,78,82,89 */
+int vgen_resize_bicubic_crop_normalize(const uint8_t* src, int64_t n, int64_t h, int64_t w, const int32_t* hbounds,
+                                       const int32_t* hcoef, int64_t kh, const int32_t* vbounds, const int32_t* vcoef,
+                                       int64_t kv, int64_t ch, int64_t cw, int64_t tile_rows, const float* mean3,
+                                       const float* std3, void* out, int out_f32, void* stream);
+/* The four scores of one video from fp32 features: clip_frames [f][e], text [e], clip_targets [t][e], dino_frames [f][d],
+ * dino_targets [t][d] (t may be 0).  Rows are L2-normalised (x / max(||x||, 1e-12)); the frame means are not re-normalised.
+ * out4 fp32 = {CLIP-T, CLIP-I, DINO-I, temporal consistency}; t = 0 gives CLIP-I = DINO-I = 0, f = 1 a NaN temporal
+ * consistency (the mean of an empty tensor).  One block; (3f + 4t + e + d + 1) floats must fit in 48 KB.
+ * replaces: cal_metric_DreamVideo.py:65,74,85,94-124 */
+int vgen_video_scores(const float* clip_frames, int64_t f, int64_t e, const float* text, const float* clip_targets,
+                      int64_t t, const float* dino_frames, const float* dino_targets, int64_t d, float* out4, void* stream);
 
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */

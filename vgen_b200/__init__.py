@@ -5,7 +5,8 @@ AutoencoderKL.decode, exposed under the reference's MODEL / DIFFUSION / AUTO_ENC
 the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`) and sketch annotators (`PiDiNet` / `pidinet_bsd`,
 `SketchSimplification` / `sketch_simplification_gan`), and DreamVideo's textual-inversion text path
 (`FrozenOpenCLIPCustomEmbedder` + `EmbeddingManager`, EMBEDDER / EMBEDMANAGER) with DDIM inversion
-(`DiffusionDDIM.ddim_reverse_sample_loop`).
+(`DiffusionDDIM.ddim_reverse_sample_loop`), and DreamVideo's evaluation metric (`calculate_metric`, `score_video`,
+`load_clip`, `dino_transform`, with the DINO ViT `vit_small`).
 
 Every op of the path is a hand-written CUDA kernel in libvgen_b200.so (include/vgen_b200.h); this
 package holds only the host-side mirror of the reference interface.  There is no CPU / PyTorch
@@ -41,6 +42,12 @@ def __getattr__(name):  # lazy: importing the package must not require torch.cud
     if name in ("PiDiNet", "pidinet_bsd", "SketchSimplification", "sketch_simplification_gan"):
         from . import sketch
         return getattr(sketch, name)
+    if name in ("calculate_metric", "score_video", "load_clip", "dino_transform"):
+        from . import metric
+        return getattr(metric, name)
+    if name in ("vit_tiny", "vit_small", "vit_base"):
+        from . import dino
+        return getattr(dino, name)
     if name == "LCMScheduler":
         from .lcm import LCMScheduler
         return LCMScheduler

@@ -69,6 +69,9 @@ class ClipModel(SpecModule):
     def __init__(self, cfg, text=True, visual=True):
         super().__init__()
         self.cfg, self.has_text, self.has_visual = cfg, text, visual
+        self.act = cfg.get("act", "gelu")            # MLP activation: "gelu" (open_clip ViT-H) or "quick_gelu" (OpenAI)
+        if self.act not in ("gelu", "quick_gelu"):
+            raise ValueError(f"vgen_b200 CLIP: act must be 'gelu' or 'quick_gelu', got {self.act!r}")
         self._build_params(clip_spec(cfg, text, visual))
         with torch.no_grad():
             self.logit_scale.fill_(2.6592)
@@ -116,7 +119,7 @@ class ClipModel(SpecModule):
 
     # ---- one residual block (ResidualAttentionBlock.forward) -------------------------------------
     @staticmethod
-    def _block(x, W, p, heads, causal):
+    def _block(x, W, p, heads, causal, act="gelu"):
         b, L, w = x.shape
         x2 = x.view(b * L, w)
         h = ops.layer_norm(x2, W[p + "ln_1.g"], W[p + "ln_1.b"])
@@ -124,7 +127,7 @@ class ClipModel(SpecModule):
         a = ops.attention_cross_small(qkv[:, :, :w], qkv[:, :, w:2 * w], qkv[:, :, 2 * w:], heads, causal=causal)
         x2 = ops.linear(a.view(b * L, w), W[p + "out.w"], bias=W[p + "out.b"], residual=x2)
         h = ops.layer_norm(x2, W[p + "ln_2.g"], W[p + "ln_2.b"])
-        h = ops.eltwise("gelu", ops.linear(h, W[p + "fc.w"], bias=W[p + "fc.b"]))
+        h = ops.eltwise(act, ops.linear(h, W[p + "fc.w"], bias=W[p + "fc.b"]))
         return ops.linear(h, W[p + "proj.w"], bias=W[p + "proj.b"], residual=x2).view(b, L, w)
 
     # ---- towers ----------------------------------------------------------------------------------
@@ -148,7 +151,7 @@ class ClipModel(SpecModule):
         else:
             x = ops.embed_tokens_extra(tokens.contiguous(), W["tok"], extra, W["pos"], check=False)
         for i in range(t["layers"] - int(layer_idx)):
-            x = self._block(x, W, f"transformer.resblocks.{i}.", t["heads"], True)
+            x = self._block(x, W, f"transformer.resblocks.{i}.", t["heads"], True, self.act)
         b, L, w = x.shape
         return ops.layer_norm(x.view(b * L, w), W["ln_final.g"], W["ln_final.b"]).view(b, L, w)
 
@@ -169,16 +172,31 @@ class ClipModel(SpecModule):
         """image [b, 3, H, W] (preprocessed, CUDA) -> fp32 [b, E]."""
         if not image.is_cuda:
             raise ops._l.VgenError("vgen_b200 CLIP: image must be a CUDA tensor (no CPU path exists)")
-        W = self._packed or self._pack()
-        v = self.cfg["vision_cfg"]
+        self._packed or self._pack()
         b, c, H, Wd = image.shape
+        img = ops.cp_to_pc(image.float().contiguous(), b, c, H * Wd).view(b, H, Wd, c)              # channels-last fp16
+        return self._image_tower(img).float()
+
+    @graphed
+    @torch.no_grad()
+    def encode_image_nhwc(self, image):
+        """image fp16 channels-last [b, H, W, 3] (preprocessed, CUDA; e.g. ops.resize_crop_normalize) -> fp32 [b, E]."""
+        if not image.is_cuda or image.dtype != torch.float16 or image.dim() != 4 or image.shape[3] != 3:
+            raise ops._l.VgenError("vgen_b200 CLIP: image must be a CUDA fp16 tensor [b, H, W, 3] (no CPU path exists)")
+        self._packed or self._pack()
+        y = self._image_tower(image.contiguous())
+        return ops.pc_to_cp(y.view(y.shape[0], 1, y.shape[1]), y.shape[0], y.shape[1], 1, torch.float32).view(y.shape)
+
+    def _image_tower(self, img):
+        W = self._packed
+        v = self.cfg["vision_cfg"]
+        b, H, Wd, c = img.shape
         ps, wv = v["patch_size"], v["width"]
         gh, gw = H // ps, Wd // ps
-        img = ops.cp_to_pc(image.float().contiguous(), b, c, H * Wd).view(b, H, Wd, c)              # channels-last fp16
         col = ops.im2col(img, ps, ps, ps, 0, 0, gh, gw, W["visual.conv1.w"].shape[1])
         patches = ops.linear(col, W["visual.conv1.w"]).view(b, gh * gw, wv)
         L = gh * gw + 1
-        x = torch.empty(b, L, wv, device=image.device, dtype=torch.float16)
+        x = torch.empty(b, L, wv, device=img.device, dtype=torch.float16)
         xr = x.view(b, L * wv)
         ops.copy2d(W["visual.cls"].expand(b, wv), xr[:, :wv])
         ops.copy2d(patches.view(b, gh * gw * wv), xr[:, wv:])
@@ -186,9 +204,49 @@ class ClipModel(SpecModule):
         x = ops.layer_norm(x.view(b * L, wv), W["visual.ln_pre.g"], W["visual.ln_pre.b"]).view(b, L, wv)
         heads = wv // v["head_width"]
         for i in range(v["layers"]):
-            x = self._block(x, W, f"visual.transformer.resblocks.{i}.", heads, False)
-        pooled = ops.layer_norm(x[:, 0].contiguous(), W["visual.ln_post.g"], W["visual.ln_post.b"])
-        return ops.linear_small(pooled, W["visual.proj.w"]).float()
+            x = self._block(x, W, f"visual.transformer.resblocks.{i}.", heads, False, self.act)
+        pooled = ops.layer_norm(x.view(b, L * wv)[:, :wv], W["visual.ln_post.g"], W["visual.ln_post.b"])   # class tokens
+        return ops.linear_small(pooled, W["visual.proj.w"])
+
+
+def openai_cfg(sd):
+    """The cfg of an OpenAI-format CLIP state dict, derived as build_model_from_openai_state_dict does
+    (utils/reward/open_clip/model.py:354-397): widths, layer counts, patch size, grid, context length and vocabulary from
+    the tensor shapes, heads = width // 64 in both towers, QuickGELU.  ModifiedResNet checkpoints raise."""
+    if "visual.proj" not in sd:
+        raise NotImplementedError("vgen_b200 CLIP: only the ViT CLIP models are supported; this state dict is a "
+                                  "ModifiedResNet one (RN50, RN101, ...)")
+    vw, ps = sd["visual.conv1.weight"].shape[0], sd["visual.conv1.weight"].shape[-1]
+    grid = round((sd["visual.positional_embedding"].shape[0] - 1) ** 0.5)
+    tw = sd["ln_final.weight"].shape[0]
+    return dict(embed_dim=sd["text_projection"].shape[1], act="quick_gelu",
+                vision_cfg=dict(image_size=ps * grid, patch_size=ps, width=vw, head_width=64,
+                                layers=len([k for k in sd if k.startswith("visual.") and k.endswith(".attn.in_proj_weight")])),
+                text_cfg=dict(context_length=sd["positional_embedding"].shape[0], vocab_size=sd["token_embedding.weight"].shape[0],
+                              width=tw, heads=tw // 64,
+                              layers=len({k.split(".")[2] for k in sd if k.startswith("transformer.resblocks")})))
+
+
+class OpenAIClipModel(ClipModel):
+    """OpenAI's CLIP as `clip.load` returns it (vgen_b200.metric.load_clip builds it): encode_text(ids [b, 77]) and
+    encode_image(images [b, 3, H, W]) -> fp32 [b, E]."""
+
+    def __init__(self, cfg):
+        super().__init__(cfg, text=True, visual=True)
+
+    @torch.no_grad()
+    def encode_text(self, tokens):
+        """The pooled end-of-text position is found on the host (ids are host data), so the device runs library kernels
+        only: the text tower, one row copy per prompt, the projection and the fp32 conversion."""
+        ids = tokens.detach().to("cpu", torch.int64)
+        eot = ids.argmax(dim=-1).tolist()
+        x = self.text_tokens(ids.to(self.device))
+        b, L, w = x.shape
+        pooled = torch.empty(b, w, device=x.device, dtype=torch.float16)
+        for i, e in enumerate(eot):
+            ops.copy2d(x[i, e:e + 1], pooled[i:i + 1])
+        xt = ops.linear_small(pooled, self._packed["text_projection.w"])
+        return ops.pc_to_cp(xt.view(b, 1, -1), b, xt.shape[1], 1, torch.float32).view(b, -1)
 
 
 class _EmbedderBase(nn.Module):

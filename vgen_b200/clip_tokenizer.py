@@ -122,13 +122,15 @@ class ClipTokenizer:
             out.extend(self.ids[p] for p in self._merge_word(word))
         return out
 
-    def __call__(self, texts, context_length=CONTEXT_LENGTH):
+    def __call__(self, texts, context_length=CONTEXT_LENGTH, truncate=True):
         if isinstance(texts, str):
             texts = [texts]
         res = torch.zeros(len(texts), context_length, dtype=torch.long)
         for i, t in enumerate(texts):
             ids = [self.sot] + self.encode(t) + [self.eot]
             if len(ids) > context_length:
+                if not truncate:             # OpenAI clip.tokenize(truncate=False)
+                    raise RuntimeError(f"Input {t} is too long for context length {context_length}")
                 ids = ids[:context_length]
                 ids[-1] = self.eot
             res[i, :len(ids)] = torch.tensor(ids)
@@ -138,9 +140,10 @@ class ClipTokenizer:
 _DEFAULT = None
 
 
-def tokenize(texts, context_length=CONTEXT_LENGTH):
-    """Drop-in for open_clip.tokenize."""
+def tokenize(texts, context_length=CONTEXT_LENGTH, truncate=True):
+    """Drop-in for open_clip.tokenize; truncate=False is OpenAI's clip.tokenize default: a text longer than
+    context_length - 2 BPE tokens raises RuntimeError instead of being cut."""
     global _DEFAULT
     if _DEFAULT is None:
         _DEFAULT = ClipTokenizer()
-    return _DEFAULT(texts, context_length)
+    return _DEFAULT(texts, context_length, truncate)

@@ -144,6 +144,14 @@ __global__ void eltwise_kernel(const __half* __restrict__ a, const __half* __res
   }
   y[idx] = __float2half_rn(r);
 }
+// op 6: QuickGELU x * sigmoid(1.702 x) (OpenAI CLIP's activation, open_clip transformer.py QuickGELU); its own kernel, so
+// the ops above keep their code
+__global__ void quick_gelu_kernel(const __half* __restrict__ a, __half* __restrict__ y, long n) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const float x = __half2float(a[idx]);
+  y[idx] = __float2half_rn(x / (1.0f + expf(-1.702f * x)));
+}
 
 // ------------------------------------------------------------------ small linear (M rows small or K tiny)
 // out[m][n] = (act_in(a[m][:]) . w[n][:] + bias[n]) (+ res[m][n]); one warp per output element.
@@ -384,9 +392,15 @@ int vgen_copy2d(const void* src, int64_t lds, void* dst, int64_t ldd, int64_t ro
 }
 
 int vgen_eltwise(int op, const void* a, const void* b, void* y, int64_t n, float s, void* stream) {
-  VG_REQUIRE(a && y && op >= 0 && op <= 5, "vgen_eltwise: bad arguments");
+  VG_REQUIRE(a && y && op >= 0 && op <= 6, "vgen_eltwise: bad arguments");
   VG_REQUIRE(!(op == 1 || op == 4) || b, "vgen_eltwise: binary op needs b");
   if (n == 0) return 0;
+  if (op == 6) {
+    launch_kernel(quick_gelu_kernel, dim3(nblk(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
+                  reinterpret_cast<const __half*>(a), reinterpret_cast<__half*>(y), n);
+    VG_LAUNCH_CHECK("quick_gelu_kernel");
+    return 0;
+  }
   launch_kernel(eltwise_kernel, dim3(nblk(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), 
       reinterpret_cast<const __half*>(a), reinterpret_cast<const __half*>(b), reinterpret_cast<__half*>(y), n, op, s);
   VG_LAUNCH_CHECK("eltwise_kernel");

@@ -1,0 +1,199 @@
+"""H100-native DINO ViT: a drop-in for DreamVideo's metric/dino/vision_transformer.py (`VisionTransformer`, `vit_tiny`,
+`vit_small`, `vit_base`), the DINO-I feature extractor of metric/cal_metric_DreamVideo.py.
+
+Same constructor arguments and state-dict names, so `dino_deitsmall16_pretrain.pth` loads into `vit_small()` with
+`strict=True`.  The forward is the reference's at its trained grid:
+
+  patch embedding (conv p x p, stride p, with bias) -> [CLS] + pos_embed -> depth x pre-LN blocks (LayerNorm eps of the
+  norm_layer, qkv with bias, softmax attention, proj; fc1 -> GELU(erf) -> fc2) -> norm -> class token
+
+and returns fp32 [n, embed_dim].  Every op is a kernel of libvgen_b200.so: im2col + the wgmma tap-GEMM for the patch
+embedding and the linears (bias and residual in the epilogue), LayerNorm, the head_dim-64 flash attention.  Activations
+are fp16 with fp32 accumulation and statistics; the forward is CUDA-graphed per input signature (n, H, W).
+
+Not provided: inputs whose patch grid differs from the trained one (interpolate_pos_encoding), get_last_selfattention,
+get_intermediate_layers and DINOHead raise NotImplementedError.  There is no CPU path: a CPU tensor or a CPU-resident
+model raises VgenError.
+"""
+from __future__ import annotations
+
+import functools
+
+import torch
+import torch.nn as nn
+
+from . import ops
+from .graph import graphed
+from .params import SpecModule
+
+
+def _ln_eps(norm_layer):
+    if norm_layer is nn.LayerNorm:
+        return 1e-5
+    if isinstance(norm_layer, functools.partial) and norm_layer.func is nn.LayerNorm and not norm_layer.args:
+        return float(norm_layer.keywords.get("eps", 1e-5))
+    raise NotImplementedError(f"vgen_b200 DINO: norm_layer must be nn.LayerNorm or a partial of it, got {norm_layer!r}")
+
+
+def dino_spec(img_size, patch_size, in_chans, num_classes, embed_dim, depth, mlp_ratio, qkv_bias):
+    """(name, shape) in the order of the reference VisionTransformer's state_dict()."""
+    D, hid = embed_dim, int(embed_dim * mlp_ratio)
+    n = (img_size // patch_size) ** 2
+    spec = [("cls_token", (1, 1, D)), ("pos_embed", (1, n + 1, D)),
+            ("patch_embed.proj.weight", (D, in_chans, patch_size, patch_size)), ("patch_embed.proj.bias", (D,))]
+    for i in range(depth):
+        p = f"blocks.{i}."
+        spec += [(p + "norm1.weight", (D,)), (p + "norm1.bias", (D,)), (p + "attn.qkv.weight", (3 * D, D))]
+        if qkv_bias:
+            spec += [(p + "attn.qkv.bias", (3 * D,))]
+        spec += [(p + "attn.proj.weight", (D, D)), (p + "attn.proj.bias", (D,)), (p + "norm2.weight", (D,)),
+                 (p + "norm2.bias", (D,)), (p + "mlp.fc1.weight", (hid, D)), (p + "mlp.fc1.bias", (hid,)),
+                 (p + "mlp.fc2.weight", (D, hid)), (p + "mlp.fc2.bias", (D,))]
+    spec += [("norm.weight", (D,)), ("norm.bias", (D,))]
+    if num_classes > 0:
+        spec += [("head.weight", (num_classes, D)), ("head.bias", (num_classes,))]
+    return spec
+
+
+class VisionTransformer(SpecModule):
+    """metric/dino/vision_transformer.py VisionTransformer (inference forward only)."""
+
+    def __init__(self, img_size=(224,), patch_size=16, in_chans=3, num_classes=0, embed_dim=768, depth=12, num_heads=12,
+                 mlp_ratio=4., qkv_bias=False, qk_scale=None, drop_rate=0., attn_drop_rate=0., drop_path_rate=0.,
+                 norm_layer=nn.LayerNorm, **kwargs):
+        super().__init__()
+        if embed_dim % num_heads or embed_dim // num_heads != 64:
+            raise NotImplementedError(f"vgen_b200 DINO: head_dim {embed_dim / num_heads:g} (the attention kernel serves "
+                                      "head_dim 64, as in vit_tiny / vit_small / vit_base)")
+        self.num_features = self.embed_dim = embed_dim
+        self.img_size, self.patch_size, self.in_chans = int(img_size[0]), int(patch_size), int(in_chans)
+        self.depth, self.num_heads, self.mlp_ratio, self.qkv_bias = depth, num_heads, mlp_ratio, qkv_bias
+        self.scale = qk_scale or (embed_dim // num_heads) ** -0.5
+        self.eps = _ln_eps(norm_layer)
+        self.num_patches = (self.img_size // self.patch_size) ** 2
+        self._build_params(dino_spec(self.img_size, self.patch_size, in_chans, num_classes, embed_dim, depth, mlp_ratio,
+                                     qkv_bias))
+        with torch.no_grad():
+            self.cls_token.normal_(std=0.02, generator=torch.Generator().manual_seed(1))
+            self.pos_embed.normal_(std=0.02, generator=torch.Generator().manual_seed(2))
+
+    # ---- packing -------------------------------------------------------------------------------
+    def _pack(self):
+        dev = self.device
+        if dev.type != "cuda":
+            raise ops._l.VgenError("vgen_b200 DINO forward needs the model on a CUDA device (no CPU path exists)")
+        sd = self.state_dict()
+        f16 = lambda t: t.detach().to(device=dev, dtype=torch.float16).contiguous()  # noqa: E731
+        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
+        W = {}
+        w = sd["patch_embed.proj.weight"]                                     # [D, c, p, p] -> [D, (ky, kx, c)] K-padded
+        k = w.shape[1] * w.shape[2] * w.shape[3]
+        wp = torch.zeros(w.shape[0], ((k + 63) // 64) * 64)
+        wp[:, :k] = w.detach().float().cpu().permute(0, 2, 3, 1).reshape(w.shape[0], k)
+        W["patch.w"], W["patch.b"] = f16(wp), f32(sd["patch_embed.proj.bias"])
+        W["cls"], W["pos"] = f16(sd["cls_token"].reshape(1, -1)), f32(sd["pos_embed"].reshape(-1))
+        for i in range(self.depth):
+            p = f"blocks.{i}."
+            for nm in ("norm1.", "norm2."):
+                W[p + nm + "g"], W[p + nm + "b"] = f32(sd[p + nm + "weight"]), f32(sd[p + nm + "bias"])
+            W[p + "qkv.w"] = f16(sd[p + "attn.qkv.weight"])
+            W[p + "qkv.b"] = f32(sd[p + "attn.qkv.bias"]) if self.qkv_bias else None
+            for nm, src in (("proj.", "attn.proj."), ("fc1.", "mlp.fc1."), ("fc2.", "mlp.fc2.")):
+                W[p + nm + "w"], W[p + nm + "b"] = f16(sd[p + src + "weight"]), f32(sd[p + src + "bias"])
+        W["norm.g"], W["norm.b"] = f32(sd["norm.weight"]), f32(sd["norm.bias"])
+        self._packed = W
+        return W
+
+    # ---- forward -------------------------------------------------------------------------------
+    def _check_grid(self, H, Wd):
+        p = self.patch_size
+        if H != Wd or (H // p) * (Wd // p) != self.num_patches:
+            raise NotImplementedError(f"vgen_b200 DINO: a {H}x{Wd} input has a different patch grid from the trained "
+                                      f"{self.img_size}x{self.img_size} one (interpolate_pos_encoding is not provided)")
+
+    def forward(self, x):
+        """x [n, in_chans, H, W] (CUDA; H = W at the trained grid) -> fp32 [n, embed_dim]."""
+        if not torch.is_tensor(x) or x.dim() != 4 or x.shape[1] != self.in_chans:
+            raise ValueError(f"vgen_b200 DINO: expected a tensor [n, {self.in_chans}, H, W], got {getattr(x, 'shape', x)}")
+        self._check_grid(x.shape[2], x.shape[3])
+        if not x.is_cuda:
+            raise ops._l.VgenError("vgen_b200 DINO: input must be a CUDA tensor (no CPU path exists)")
+        return self._forward_nchw(x.float().contiguous())
+
+    def forward_nhwc(self, img):
+        """img fp16 channels-last [n, H, W, in_chans] (CUDA, e.g. ops.resize_crop_normalize's output) -> fp32 [n, D]."""
+        if not img.is_cuda or img.dtype != torch.float16 or img.dim() != 4 or img.shape[3] != self.in_chans:
+            raise ops._l.VgenError(f"vgen_b200 DINO: expected a CUDA fp16 tensor [n, H, W, {self.in_chans}]")
+        self._check_grid(img.shape[1], img.shape[2])
+        return self._forward_nhwc(img.contiguous())
+
+    @graphed
+    @torch.no_grad()
+    def _forward_nchw(self, x):
+        self._packed or self._pack()
+        n, c, H, Wd = x.shape
+        return self._tower(ops.cp_to_pc(x, n, c, H * Wd).view(n, H, Wd, c))
+
+    @graphed
+    @torch.no_grad()
+    def _forward_nhwc(self, img):
+        self._packed or self._pack()
+        return self._tower(img)
+
+    def _tower(self, img):
+        W = self._packed
+        n, H, Wd, _ = img.shape
+        p, D, eps = self.patch_size, self.embed_dim, self.eps
+        gh, gw = H // p, Wd // p
+        col = ops.im2col(img, p, p, p, 0, 0, gh, gw, W["patch.w"].shape[1])
+        patches = ops.linear(col, W["patch.w"], bias=W["patch.b"])
+        L = gh * gw + 1
+        x = torch.empty(n, L, D, device=img.device, dtype=torch.float16)
+        xr = x.view(n, L * D)
+        ops.copy2d(W["cls"].expand(n, D), xr[:, :D])
+        ops.copy2d(patches.view(n, gh * gw * D), xr[:, D:])
+        ops.add_rows_f32_(x, W["pos"])
+        x2 = x.view(n * L, D)
+        for i in range(self.depth):
+            q = f"blocks.{i}."
+            h = ops.layer_norm(x2, W[q + "norm1.g"], W[q + "norm1.b"], eps)
+            qkv = ops.linear(h, W[q + "qkv.w"], bias=W[q + "qkv.b"]).view(n, L, 3 * D)
+            a = ops.attention_d64(qkv[:, :, :D], qkv[:, :, D:2 * D], qkv[:, :, 2 * D:], self.num_heads, scale=self.scale)
+            x2 = ops.linear(a.view(n * L, D), W[q + "proj.w"], bias=W[q + "proj.b"], residual=x2)
+            h = ops.layer_norm(x2, W[q + "norm2.g"], W[q + "norm2.b"], eps)
+            h = ops.eltwise("gelu", ops.linear(h, W[q + "fc1.w"], bias=W[q + "fc1.b"]))
+            x2 = ops.linear(h, W[q + "fc2.w"], bias=W[q + "fc2.b"], residual=x2)
+        y = ops.layer_norm(x2.view(n, L * D)[:, :D], W["norm.g"], W["norm.b"], eps)     # the class tokens
+        return ops.pc_to_cp(y.view(n, 1, D), n, D, 1, torch.float32).view(n, D)
+
+    # ---- not provided ---------------------------------------------------------------------------
+    def get_last_selfattention(self, x):
+        raise NotImplementedError("vgen_b200 DINO: get_last_selfattention is not provided (the metric uses forward only)")
+
+    def get_intermediate_layers(self, x, n=1):
+        raise NotImplementedError("vgen_b200 DINO: get_intermediate_layers is not provided (the metric uses forward only)")
+
+    def interpolate_pos_encoding(self, x, w, h):
+        raise NotImplementedError("vgen_b200 DINO: interpolate_pos_encoding is not provided (inputs must be at the trained grid)")
+
+
+def vit_tiny(patch_size=16, **kwargs):
+    return VisionTransformer(patch_size=patch_size, embed_dim=192, depth=12, num_heads=3, mlp_ratio=4, qkv_bias=True,
+                             norm_layer=functools.partial(nn.LayerNorm, eps=1e-6), **kwargs)
+
+
+def vit_small(patch_size=16, **kwargs):
+    return VisionTransformer(patch_size=patch_size, embed_dim=384, depth=12, num_heads=6, mlp_ratio=4, qkv_bias=True,
+                             norm_layer=functools.partial(nn.LayerNorm, eps=1e-6), **kwargs)
+
+
+def vit_base(patch_size=16, **kwargs):
+    return VisionTransformer(patch_size=patch_size, embed_dim=768, depth=12, num_heads=12, mlp_ratio=4, qkv_bias=True,
+                             norm_layer=functools.partial(nn.LayerNorm, eps=1e-6), **kwargs)
+
+
+class DINOHead(nn.Module):
+    """The self-distillation projection head (training only): not provided."""
+
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError("vgen_b200 DINO: DINOHead (training / evaluation head) is not provided")

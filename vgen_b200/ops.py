@@ -348,9 +348,9 @@ def fold_layer_norm(w, bias, gamma, beta):
 
 # ------------------------------------------------------------------------------------------------
 # attention
-def attention_d64(q, k, v, heads, kv_batch_div=1, out=None):
+def attention_d64(q, k, v, heads, kv_batch_div=1, out=None, scale=None):
     """q [b, lq, heads*64] (last-dim-contiguous views allowed, e.g. slices of a fused qkv buffer),
-    k/v [b // kv_batch_div, lk, heads*64] -> out [b, lq, heads*64]."""
+    k/v [b // kv_batch_div, lk, heads*64] -> out [b, lq, heads*64].  scale: the softmax scale (None: 64 ** -0.5)."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _chk16(t, nm)
         if t.dim() != 3 or t.stride(2) != 1 or t.stride(0) != t.shape[1] * t.stride(1):
@@ -363,7 +363,8 @@ def attention_d64(q, k, v, heads, kv_batch_div=1, out=None):
         out = torch.empty(b, lq, inner, device=q.device, dtype=torch.float16)
     rc = _run("attention_d64", 4.0 * b * heads * lq * lk * 64, 2.0 * (2 * b * lq * inner + 2 * k.shape[0] * lk * inner),
               lambda: _l.load().vgen_attention_d64(_p(q), _p(k), _p(v), _p(out), b, heads, lq, lk, q.stride(1), k.stride(1),
-                                                   v.stride(1), out.stride(1), kv_batch_div, 64 ** -0.5, _stream()),
+                                                   v.stride(1), out.stride(1), kv_batch_div,
+                                                   64 ** -0.5 if scale is None else float(scale), _stream()),
               tag=f"b{b} h{heads} lq{lq} lk{lk}")
     _l.check(rc, "vgen_attention_d64")
     return out
@@ -559,7 +560,7 @@ def concat_channels(a, b):
     return out
 
 
-_ELT = {"silu": 0, "add": 1, "gelu": 2, "scale": 3, "axpy": 4, "relu": 5}
+_ELT = {"silu": 0, "add": 1, "gelu": 2, "scale": 3, "axpy": 4, "relu": 5, "quick_gelu": 6}
 
 
 def eltwise(op, a, b=None, s=1.0, out=None):
@@ -956,3 +957,50 @@ def sketch_normalize(x, mean, std):
                                          _p(y), _stream())
     _l.check(rc, "vgen_sketch_normalize")
     return y
+
+
+# ------------------------------------------------------------------------------------------------
+# DreamVideo's evaluation metric (metric.cu)
+def resize_crop_normalize(images, plan, out_f32=False, out=None):
+    """Pillow-exact bicubic resize + centre crop + normalisation of uint8 images [n, h, w, 3] (contiguous, CUDA) with the
+    fixed-point tables of `plan` (metric.ResizePlan, moved to the images' device) -> fp16 [n, crop_h, crop_w, 3] or, with
+    out_f32, fp32 [n, 3, crop_h, crop_w]; `out` (contiguous, that shape and dtype) receives it if given."""
+    if images.dtype != torch.uint8 or not images.is_cuda or not images.is_contiguous() or images.dim() != 4 or images.shape[3] != 3:
+        raise _l.VgenError("resize_crop_normalize: images must be a contiguous CUDA uint8 tensor [n, h, w, 3]")
+    n, h, w, _ = images.shape
+    if (h, w) != (plan.h, plan.w):
+        raise _l.VgenError(f"resize_crop_normalize: the plan is for {plan.h}x{plan.w} images, got {h}x{w}")
+    hb, hk, vb, vk = plan.tables(images.device)
+    ch, cw = plan.crop_h, plan.crop_w
+    shape, dtype = ((n, 3, ch, cw), torch.float32) if out_f32 else ((n, ch, cw, 3), torch.float16)
+    if out is None:
+        out = torch.empty(shape, device=images.device, dtype=dtype)
+    elif tuple(out.shape) != shape or out.dtype != dtype or not out.is_contiguous() or out.device != images.device:
+        raise _l.VgenError(f"resize_crop_normalize: out must be a contiguous {dtype} tensor {list(shape)} on {images.device}")
+    m3 = (ctypes.c_float * 3)(*[float(v) for v in plan.mean])
+    s3 = (ctypes.c_float * 3)(*[float(v) for v in plan.std])
+    rc = _run("resize_crop_norm", 0.0, images.numel() + out.numel() * out.element_size(),
+              lambda: _l.load().vgen_resize_bicubic_crop_normalize(_p(images), n, h, w, _p(hb), _p(hk), hk.shape[1], _p(vb),
+                                                                   _p(vk), vk.shape[1], ch, cw, plan.tile_rows, m3, s3,
+                                                                   _p(out), 1 if out_f32 else 0, _stream()))
+    _l.check(rc, "vgen_resize_bicubic_crop_normalize")
+    return out
+
+
+def video_scores(clip_frames, text, clip_targets, dino_frames, dino_targets):
+    """(CLIP-T, CLIP-I, DINO-I, temporal consistency) of one video as a CUDA fp32 [4] tensor, from fp32 features
+    clip_frames [f, e], text [e], dino_frames [f, d] and the targets' [t, e] / [t, d] (None or t = 0: no targets)."""
+    f, e = clip_frames.shape
+    d = dino_frames.shape[1]
+    t = 0 if clip_targets is None else clip_targets.shape[0]
+    ts = [(clip_frames, "clip_frames", (f, e)), (text, "text", (e,)), (dino_frames, "dino_frames", (f, d))]
+    if t:
+        ts += [(clip_targets, "clip_targets", (t, e)), (dino_targets, "dino_targets", (t, d))]
+    for x, nm, shape in ts:
+        if x.dtype != torch.float32 or not x.is_cuda or not x.is_contiguous() or tuple(x.shape) != shape:
+            raise _l.VgenError(f"video_scores: {nm} must be a contiguous CUDA fp32 tensor {list(shape)}")
+    out = torch.empty(4, device=clip_frames.device, dtype=torch.float32)
+    rc = _l.load().vgen_video_scores(_p(clip_frames), f, e, _p(text), _p(clip_targets) if t else None, t, _p(dino_frames),
+                                     _p(dino_targets) if t else None, d, _p(out), _stream())
+    _l.check(rc, "vgen_video_scores")
+    return out
