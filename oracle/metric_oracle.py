@@ -4,8 +4,8 @@
     ImagingResampleHorizontal_8bpc / Vertical_8bpc) in numpy integer arithmetic, and the torchvision transforms built on
     it (Resize(short side) -> CenterCrop -> ToTensor -> Normalize) in numpy float32;
   * OpenAI's CLIP (the open_clip CLIP built by build_model_from_openai_state_dict: QuickGELU in both towers), from an
-    OpenAI-format state dict;
-  * DINO's VisionTransformer (metric/dino/vision_transformer.py) with torch.nn.functional;
+    OpenAI-format state dict: oracle/clip_oracle.py's towers with QuickGELU and head width 64;
+  * DINO's VisionTransformer (metric/dino/vision_transformer.py): clip_oracle's block with DINO's names and eps;
   * the four scores of calculate_metric.
 
 tools/make_golden_metric.py checks it against the reference's own calculate_metric and freezes the results.
@@ -18,7 +18,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from .clip_oracle import _n_layers
+from . import clip_oracle
 
 PRECISION_BITS = 32 - 8 - 2
 OPENAI_MEAN, OPENAI_STD = (0.48145466, 0.4578275, 0.40821073), (0.26862954, 0.26130258, 0.27577711)
@@ -124,46 +124,20 @@ def quick_gelu(x):
     return x * torch.sigmoid(1.702 * x)
 
 
-def _clip_block(x, sd, p, heads, causal):
-    """open_clip ResidualAttentionBlock with act_layer=QuickGELU (oracle/clip_oracle.py's block with the OpenAI activation)."""
-    b, L, W = x.shape
-    d = W // heads
-    h = F.layer_norm(x, (W,), sd[p + "ln_1.weight"], sd[p + "ln_1.bias"], 1e-5)
-    q, k, v = F.linear(h, sd[p + "attn.in_proj_weight"], sd[p + "attn.in_proj_bias"]).chunk(3, dim=-1)
-    sp = lambda t: t.reshape(b, L, heads, d).permute(0, 2, 1, 3)  # noqa: E731
-    o = F.scaled_dot_product_attention(sp(q), sp(k), sp(v), is_causal=causal).permute(0, 2, 1, 3).reshape(b, L, W)
-    x = x + F.linear(o, sd[p + "attn.out_proj.weight"], sd[p + "attn.out_proj.bias"])
-    h = F.layer_norm(x, (W,), sd[p + "ln_2.weight"], sd[p + "ln_2.bias"], 1e-5)
-    h = quick_gelu(F.linear(h, sd[p + "mlp.c_fc.weight"], sd[p + "mlp.c_fc.bias"]))
-    return x + F.linear(h, sd[p + "mlp.c_proj.weight"], sd[p + "mlp.c_proj.bias"])
-
-
 def clip_encode_text(sd, tokens):
     """CLIP.encode_text: [b, 77] ids -> [b, E] (heads = width // 64, as build_model_from_openai_state_dict derives)."""
-    x = sd["token_embedding.weight"][tokens] + sd["positional_embedding"]
-    heads = x.shape[-1] // 64
-    for i in range(_n_layers(sd, "transformer.resblocks.")):
-        x = _clip_block(x, sd, f"transformer.resblocks.{i}.", heads, True)
-    x = F.layer_norm(x, (x.shape[-1],), sd["ln_final.weight"], sd["ln_final.bias"], 1e-5)
-    return x[torch.arange(x.shape[0]), tokens.argmax(dim=-1)] @ sd["text_projection"]
+    return clip_oracle.encode_text(sd, tokens, sd["ln_final.weight"].shape[0] // 64, "last", quick_gelu)[0]
 
 
 def clip_encode_image(sd, image):
     """CLIP.encode_image: [b, 3, H, W] -> [b, E]."""
-    w = sd["visual.conv1.weight"]
-    x = F.conv2d(image, w, stride=w.shape[-1])
-    b, W = x.shape[0], x.shape[1]
-    x = x.reshape(b, W, -1).permute(0, 2, 1)
-    cls = sd["visual.class_embedding"].to(x.dtype) + torch.zeros(b, 1, W, dtype=x.dtype, device=x.device)
-    x = torch.cat([cls, x], dim=1) + sd["visual.positional_embedding"]
-    x = F.layer_norm(x, (W,), sd["visual.ln_pre.weight"], sd["visual.ln_pre.bias"], 1e-5)
-    for i in range(_n_layers(sd, "visual.transformer.resblocks.")):
-        x = _clip_block(x, sd, f"visual.transformer.resblocks.{i}.", W // 64, False)
-    pooled = F.layer_norm(x[:, 0], (W,), sd["visual.ln_post.weight"], sd["visual.ln_post.bias"], 1e-5)
-    return pooled @ sd["visual.proj"]
+    return clip_oracle.encode_image(sd, image, 64, quick_gelu)
 
 
 # ---- DINO ViT ----------------------------------------------------------------------------------------------------------
+DINO_BLOCK = ("norm1.", "attn.qkv.", "attn.proj.", "norm2.", "mlp.fc1.", "mlp.fc2.")
+
+
 def dino_forward(sd, image, heads, eps=1e-6):
     """VisionTransformer.forward at the trained grid: patch embed, [CLS], + pos_embed, pre-LN blocks (qkv bias, GELU MLP),
     norm, class token -> [b, D]."""
@@ -171,18 +145,8 @@ def dino_forward(sd, image, heads, eps=1e-6):
     x = F.conv2d(image, w, sd["patch_embed.proj.bias"], stride=w.shape[-1]).flatten(2).transpose(1, 2)
     b, _, D = x.shape
     x = torch.cat([sd["cls_token"].expand(b, -1, -1), x], dim=1) + sd["pos_embed"]
-    d = D // heads
-    for i in range(_n_layers(sd, "blocks.")):
-        p = f"blocks.{i}."
-        h = F.layer_norm(x, (D,), sd[p + "norm1.weight"], sd[p + "norm1.bias"], eps)
-        qkv = F.linear(h, sd[p + "attn.qkv.weight"], sd.get(p + "attn.qkv.bias"))
-        q, k, v = qkv.reshape(b, -1, 3, heads, d).permute(2, 0, 3, 1, 4)
-        o = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(b, -1, D)
-        x = x + F.linear(o, sd[p + "attn.proj.weight"], sd[p + "attn.proj.bias"])
-        h = F.layer_norm(x, (D,), sd[p + "norm2.weight"], sd[p + "norm2.bias"], eps)
-        h = F.linear(F.gelu(F.linear(h, sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"])), sd[p + "mlp.fc2.weight"],
-                     sd[p + "mlp.fc2.bias"])
-        x = x + h
+    for i in range(clip_oracle._n_layers(sd, "blocks.")):
+        x = clip_oracle._block(x, sd, f"blocks.{i}.", heads, False, eps=eps, names=DINO_BLOCK)
     return F.layer_norm(x, (D,), sd["norm.weight"], sd["norm.bias"], eps)[:, 0]
 
 

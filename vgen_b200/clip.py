@@ -12,6 +12,7 @@ Same constructor arguments; `.model` holds the parameters under open_clip's stat
 `open_clip_pytorch_model.bin` (a plain state_dict) loads with `strict=True`; `pretrained=None` leaves random weights.
 Every op is a kernel of libvgen_b200.so: wgmma tap-GEMMs for the projections / MLPs (bias, residual in the epilogue),
 LayerNorm, the small-attention kernel (77 causal tokens at head_dim 64; 257 tokens at head_dim 80), embedding gather.
+The patch embedding and the blocks are the shared ViT trunk (vgen_b200.vit).
 The reference runs CLIP in fp32; here activations are fp16 with fp32 accumulation / statistics (the UNet consumes the
 tokens as fp16 anyway), embeddings are summed in fp32.  Tokenisation is `vgen_b200.clip_tokenizer` (bit-exact ids).
 No CPU path: a CPU-resident model raises.
@@ -21,16 +22,20 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, vit
 from .clip_tokenizer import tokenize
 from .graph import graphed
 from .params import SpecModule
+from .vit import f16, f32
 
 ARCHS = {
     # utils/reward/open_clip/model_configs/ViT-H-14.json (the only arch the released configs use)
     "ViT-H-14": dict(embed_dim=1024, vision_cfg=dict(image_size=224, layers=32, width=1280, head_width=80, patch_size=14),
                      text_cfg=dict(context_length=77, vocab_size=49408, width=1024, heads=16, layers=24)),
 }
+
+# open_clip ResidualAttentionBlock: the state-dict prefixes of LN1, qkv, proj, LN2, fc1, fc2 (vit.pack_block)
+_BLOCK = ("ln_1.", "attn.in_proj_", "attn.out_proj.", "ln_2.", "mlp.c_fc.", "mlp.c_proj.")
 
 
 def _block_spec(p, w):
@@ -82,53 +87,24 @@ class ClipModel(SpecModule):
         dev = self.device
         if dev.type != "cuda":
             raise ops._l.VgenError("vgen_b200 CLIP forward needs the model on a CUDA device (no CPU path exists)")
-        f16 = lambda t: t.detach().to(device=dev, dtype=torch.float16).contiguous()  # noqa: E731
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
         W = {}
-
-        def block(p):
-            for ln in ("ln_1.", "ln_2."):
-                W[p + ln + "g"], W[p + ln + "b"] = f32(sd[p + ln + "weight"]), f32(sd[p + ln + "bias"])
-            W[p + "qkv.w"], W[p + "qkv.b"] = f16(sd[p + "attn.in_proj_weight"]), f32(sd[p + "attn.in_proj_bias"])
-            W[p + "out.w"], W[p + "out.b"] = f16(sd[p + "attn.out_proj.weight"]), f32(sd[p + "attn.out_proj.bias"])
-            W[p + "fc.w"], W[p + "fc.b"] = f16(sd[p + "mlp.c_fc.weight"]), f32(sd[p + "mlp.c_fc.bias"])
-            W[p + "proj.w"], W[p + "proj.b"] = f16(sd[p + "mlp.c_proj.weight"]), f32(sd[p + "mlp.c_proj.bias"])
-
         if self.has_text:
-            W["tok"], W["pos"] = f32(sd["token_embedding.weight"]), f32(sd["positional_embedding"])
+            W["tok"], W["pos"] = f32(sd["token_embedding.weight"], dev), f32(sd["positional_embedding"], dev)
             for i in range(self.cfg["text_cfg"]["layers"]):
-                block(f"transformer.resblocks.{i}.")
-            W["ln_final.g"], W["ln_final.b"] = f32(sd["ln_final.weight"]), f32(sd["ln_final.bias"])
-            W["text_projection.w"] = f16(sd["text_projection"].t())                  # x @ P == linear(x, P^T)
+                vit.pack_block(W, sd, f"transformer.resblocks.{i}.", _BLOCK, dev)
+            W["ln_final.g"], W["ln_final.b"] = f32(sd["ln_final.weight"], dev), f32(sd["ln_final.bias"], dev)
+            W["text_projection.w"] = f16(sd["text_projection"].t(), dev)             # x @ P == linear(x, P^T)
         if self.has_visual:
-            v = self.cfg["vision_cfg"]
-            w = sd["visual.conv1.weight"]                                           # [wv, 3, p, p] -> [wv, (ky, kx, c)] K-padded
-            k = w.shape[2] * w.shape[3] * 3
-            kpad = ((k + 63) // 64) * 64
-            wp = torch.zeros(w.shape[0], kpad)
-            wp[:, :k] = w.detach().float().cpu().permute(0, 2, 3, 1).reshape(w.shape[0], k)
-            W["visual.conv1.w"] = f16(wp)
-            W["visual.cls"], W["visual.pos"] = f16(sd["visual.class_embedding"].reshape(1, -1)), f32(sd["visual.positional_embedding"])
-            for nm in ("ln_pre.", "ln_post."):
-                W["visual." + nm + "g"], W["visual." + nm + "b"] = f32(sd["visual." + nm + "weight"]), f32(sd["visual." + nm + "bias"])
-            for i in range(v["layers"]):
-                block(f"visual.transformer.resblocks.{i}.")
-            W["visual.proj.w"] = f16(sd["visual.proj"].t())
+            W["visual.conv1.w"] = vit.pack_patch(sd["visual.conv1.weight"], dev)
+            W["visual.cls"] = f16(sd["visual.class_embedding"].reshape(1, -1), dev)
+            W["visual.pos"] = f32(sd["visual.positional_embedding"], dev)
+            for nm in ("visual.ln_pre.", "visual.ln_post."):
+                W[nm + "g"], W[nm + "b"] = f32(sd[nm + "weight"], dev), f32(sd[nm + "bias"], dev)
+            for i in range(self.cfg["vision_cfg"]["layers"]):
+                vit.pack_block(W, sd, f"visual.transformer.resblocks.{i}.", _BLOCK, dev)
+            W["visual.proj.w"] = f16(sd["visual.proj"].t(), dev)
         self._packed = W
         return W
-
-    # ---- one residual block (ResidualAttentionBlock.forward) -------------------------------------
-    @staticmethod
-    def _block(x, W, p, heads, causal, act="gelu"):
-        b, L, w = x.shape
-        x2 = x.view(b * L, w)
-        h = ops.layer_norm(x2, W[p + "ln_1.g"], W[p + "ln_1.b"])
-        qkv = ops.linear(h, W[p + "qkv.w"], bias=W[p + "qkv.b"]).view(b, L, 3 * w)
-        a = ops.attention_cross_small(qkv[:, :, :w], qkv[:, :, w:2 * w], qkv[:, :, 2 * w:], heads, causal=causal)
-        x2 = ops.linear(a.view(b * L, w), W[p + "out.w"], bias=W[p + "out.b"], residual=x2)
-        h = ops.layer_norm(x2, W[p + "ln_2.g"], W[p + "ln_2.b"])
-        h = ops.eltwise(act, ops.linear(h, W[p + "fc.w"], bias=W[p + "fc.b"]))
-        return ops.linear(h, W[p + "proj.w"], bias=W[p + "proj.b"], residual=x2).view(b, L, w)
 
     # ---- towers ----------------------------------------------------------------------------------
     def text_tokens(self, tokens, layer_idx=0, extra=None):
@@ -151,7 +127,7 @@ class ClipModel(SpecModule):
         else:
             x = ops.embed_tokens_extra(tokens.contiguous(), W["tok"], extra, W["pos"], check=False)
         for i in range(t["layers"] - int(layer_idx)):
-            x = self._block(x, W, f"transformer.resblocks.{i}.", t["heads"], True, self.act)
+            x = vit.block(x, W, f"transformer.resblocks.{i}.", t["heads"], act=self.act, causal=True)
         b, L, w = x.shape
         return ops.layer_norm(x.view(b * L, w), W["ln_final.g"], W["ln_final.b"]).view(b, L, w)
 
@@ -190,21 +166,12 @@ class ClipModel(SpecModule):
     def _image_tower(self, img):
         W = self._packed
         v = self.cfg["vision_cfg"]
-        b, H, Wd, c = img.shape
-        ps, wv = v["patch_size"], v["width"]
-        gh, gw = H // ps, Wd // ps
-        col = ops.im2col(img, ps, ps, ps, 0, 0, gh, gw, W["visual.conv1.w"].shape[1])
-        patches = ops.linear(col, W["visual.conv1.w"]).view(b, gh * gw, wv)
-        L = gh * gw + 1
-        x = torch.empty(b, L, wv, device=img.device, dtype=torch.float16)
-        xr = x.view(b, L * wv)
-        ops.copy2d(W["visual.cls"].expand(b, wv), xr[:, :wv])
-        ops.copy2d(patches.view(b, gh * gw * wv), xr[:, wv:])
-        ops.add_rows_f32_(x, W["visual.pos"])
+        x = vit.embed(img, v["patch_size"], W["visual.conv1.w"], None, W["visual.cls"], W["visual.pos"])
+        b, L, wv = x.shape
         x = ops.layer_norm(x.view(b * L, wv), W["visual.ln_pre.g"], W["visual.ln_pre.b"]).view(b, L, wv)
         heads = wv // v["head_width"]
         for i in range(v["layers"]):
-            x = self._block(x, W, f"visual.transformer.resblocks.{i}.", heads, False, self.act)
+            x = vit.block(x, W, f"visual.transformer.resblocks.{i}.", heads, act=self.act)
         pooled = ops.layer_norm(x.view(b, L * wv)[:, :wv], W["visual.ln_post.g"], W["visual.ln_post.b"])   # class tokens
         return ops.linear_small(pooled, W["visual.proj.w"])
 

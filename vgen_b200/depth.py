@@ -10,7 +10,8 @@ whose config lists 'depthmap').
 Same constructor, parameter names, shapes and order as the reference, so `midas_v3_dpt_large.pth` loads with
 `strict=True`.  The forward takes [n, 3, H, W] on the GPU (NCHW-contiguous or channels_last) in the module's parameter
 dtype and returns [n, 1, H, W] in that dtype.  Every op is a kernel of libvgen_b200.so; activations are fp16 channels-last
-with fp32 accumulation, fp32 LayerNorm / softmax statistics.  Kernel-level notes are in DESIGN.md section 3.
+with fp32 accumulation, fp32 LayerNorm / softmax statistics.  The patch embedding and the blocks are the shared ViT
+trunk (vgen_b200.vit).  Kernel-level notes are in DESIGN.md section 3.
 No CPU path: a CPU input or a CPU-resident model raises VgenError.
 """
 from __future__ import annotations
@@ -18,11 +19,15 @@ from __future__ import annotations
 import torch
 import torch.nn.functional as F
 
-from . import ops
+from . import ops, vit
 from .graph import graphed
 from .params import SpecModule
+from .vit import f16, f32
 
 __all__ = ["MiDaS", "midas_v3"]
+
+# AttentionBlock (depth/__init__.py:57-76): the state-dict prefixes of LN1, qkv, proj, LN2, fc1, fc2 (vit.pack_block)
+_BLOCK = ("norm1.", "attn.to_qkv.", "attn.proj.", "norm2.", "mlp.0.", "mlp.2.")
 
 
 def midas_spec(image_size=384, patch_size=16, dim=1024, neck_dims=(256, 512, 1024, 1024), fusion_dim=256, num_layers=24):
@@ -86,45 +91,35 @@ class MiDaS(SpecModule):
         if dev.type != "cuda":
             raise ops._l.VgenError("vgen_b200 MiDaS forward needs the model on a CUDA device (no CPU path exists)")
         sd = self.state_dict()
-        f16 = lambda t: t.detach().to(device=dev, dtype=torch.float16).contiguous()  # noqa: E731
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
         # conv weight [co, ci, kh, kw] -> [co, (ky, kx, ci)], the tap-GEMM's K order
-        taps = lambda w: f16(w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1))  # noqa: E731
-        W = {}
-        d, p = self.dim, self.patch_size
-        k = 3 * p * p
-        wpe = torch.zeros(d, (k + 63) // 64 * 64, device=dev)
-        wpe[:, :k] = sd["patch_embedding.weight"].detach().to(device=dev, dtype=torch.float32).permute(0, 2, 3, 1).reshape(d, k)
-        W["pe.w"], W["pe.b"] = f16(wpe), f32(sd["patch_embedding.bias"])
-        W["cls"] = f16(sd["cls_embedding"].reshape(1, d))
-        W["pos_src"] = sd["pos_embedding"].detach().to(device="cpu", dtype=torch.float32).reshape(-1, d)
+        taps = lambda w: f16(w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1), dev)  # noqa: E731
+        d = self.dim
+        W = {"pe.w": vit.pack_patch(sd["patch_embedding.weight"], dev), "pe.b": f32(sd["patch_embedding.bias"], dev),
+             "cls": f16(sd["cls_embedding"].reshape(1, d), dev),
+             "pos_src": sd["pos_embedding"].detach().to(device="cpu", dtype=torch.float32).reshape(-1, d)}
         for i in range(self.num_layers):
-            b = f"blocks.{i}."
-            for nm in ("norm1", "norm2"):
-                W[b + nm + ".g"], W[b + nm + ".b"] = f32(sd[b + nm + ".weight"]), f32(sd[b + nm + ".bias"])
-            for nm, src in (("qkv", "attn.to_qkv"), ("proj", "attn.proj"), ("fc1", "mlp.0"), ("fc2", "mlp.2")):
-                W[b + nm + ".w"], W[b + nm + ".b"] = f16(sd[b + src + ".weight"]), f32(sd[b + src + ".bias"])
+            vit.pack_block(W, sd, f"blocks.{i}.", _BLOCK, dev)
         for s in range(1, 5):
             w = sd[f"fc{s}.0.weight"]
-            W[f"fc{s}.tok"], W[f"fc{s}.cls"], W[f"fc{s}.b"] = f16(w[:, :d]), f16(w[:, d:]), f32(sd[f"fc{s}.0.bias"])
-            W[f"conv{s}.0.w"], W[f"conv{s}.0.b"] = f16(sd[f"conv{s}.0.weight"].flatten(1)), f32(sd[f"conv{s}.0.bias"])
+            W[f"fc{s}.tok"], W[f"fc{s}.cls"], W[f"fc{s}.b"] = f16(w[:, :d], dev), f16(w[:, d:], dev), f32(sd[f"fc{s}.0.bias"], dev)
+            W[f"conv{s}.0.w"], W[f"conv{s}.0.b"] = f16(sd[f"conv{s}.0.weight"].flatten(1), dev), f32(sd[f"conv{s}.0.bias"], dev)
             if s in (1, 2):
-                W[f"conv{s}.1.w"] = f16(ops.pack_conv_transpose_weight(sd[f"conv{s}.1.weight"]))
-                W[f"conv{s}.1.b"] = f32(sd[f"conv{s}.1.bias"])
+                W[f"conv{s}.1.w"] = f16(ops.pack_conv_transpose_weight(sd[f"conv{s}.1.weight"]), dev)
+                W[f"conv{s}.1.b"] = f32(sd[f"conv{s}.1.bias"], dev)
                 W[f"conv{s}.2.w"] = taps(sd[f"conv{s}.2.weight"])
             elif s == 3:
                 W["conv3.1.w"] = taps(sd["conv3.1.weight"])
             else:
-                W["conv4.1.w"], W["conv4.1.b"] = taps(sd["conv4.1.weight"]), f32(sd["conv4.1.bias"])
+                W["conv4.1.w"], W["conv4.1.b"] = taps(sd["conv4.1.weight"]), f32(sd["conv4.1.bias"], dev)
                 W["conv4.2.w"] = taps(sd["conv4.2.weight"])
             for nm in ("layer1.residual.1", "layer1.residual.3", "layer2.residual.1", "layer2.residual.3"):
                 q = f"fusion{s}.{nm}"
-                W[q + ".w"], W[q + ".b"] = taps(sd[q + ".weight"]), f32(sd[q + ".bias"])
+                W[q + ".w"], W[q + ".b"] = taps(sd[q + ".weight"]), f32(sd[q + ".bias"], dev)
             q = f"fusion{s}.conv_out"
-            W[q + ".w"], W[q + ".b"] = f16(sd[q + ".weight"].flatten(1)), f32(sd[q + ".bias"])
+            W[q + ".w"], W[q + ".b"] = f16(sd[q + ".weight"].flatten(1), dev), f32(sd[q + ".bias"], dev)
         for nm in ("head.0", "head.2"):
-            W[nm + ".w"], W[nm + ".b"] = taps(sd[nm + ".weight"]), f32(sd[nm + ".bias"])
-        W["head.4.w"], W["head.4.b"] = f32(sd["head.4.weight"].reshape(-1)), f32(sd["head.4.bias"])
+            W[nm + ".w"], W[nm + ".b"] = taps(sd[nm + ".weight"]), f32(sd[nm + ".bias"], dev)
+        W["head.4.w"], W["head.4.b"] = f32(sd["head.4.weight"].reshape(-1), dev), f32(sd["head.4.bias"], dev)
         self._packed = W
         return W
 
@@ -172,20 +167,13 @@ class MiDaS(SpecModule):
     def _forward_nhwc(self, img, out_f32):
         W = self._packed
         n, H, Wd, _ = img.shape
-        p, d = self.patch_size, self.dim
+        p = self.patch_size
         hp, wp = H // p, Wd // p
-        L = hp * wp + 1
-        col = ops.im2col(img, p, p, p, 0, 0, hp, wp, W["pe.w"].shape[1])
-        patches = ops.linear(col, W["pe.w"], bias=W["pe.b"])
-        x = torch.empty(n, L, d, device=img.device, dtype=torch.float16)
-        xr = x.view(n, L * d)
-        ops.copy2d(W["cls"].expand(n, d), xr[:, :d])
-        ops.copy2d(patches.view(n, hp * wp * d), xr[:, d:])
-        ops.add_rows_f32_(x, self._pos(W, hp, wp))
+        x = vit.embed(img, p, W["pe.w"], W["pe.b"], W["cls"], self._pos(W, hp, wp))
         feats = []
         for s, sl in enumerate(self.slices, 1):
             for i in range(sl.start, sl.stop):
-                x = self._block(x, W, f"blocks.{i}.")
+                x = vit.block(x, W, f"blocks.{i}.", self.num_heads, attention="d64")
             feats.append(self._neck(s, self._readout(x, W, s, hp, wp), W, n, hp, wp))
         y = self._fusion(W, 4, feats[3])
         for s in (3, 2, 1):
@@ -194,18 +182,6 @@ class MiDaS(SpecModule):
         h = ops.conv2d_3x3(ops.upsample_bilinear2x(h), W["head.2.w"], bias=W["head.2.b"])
         out = ops.dpt_head_out(h, W["head.4.w"], W["head.4.b"], torch.float32 if out_f32 else torch.float16)
         return out.view(n, 1, H, Wd)
-
-    def _block(self, x, W, b):
-        """AttentionBlock (depth/__init__.py:57-76): x + attn(norm1(x)), then x + mlp(norm2(x))."""
-        n, L, d = x.shape
-        x2 = x.view(n * L, d)
-        h = ops.layer_norm(x2, W[b + "norm1.g"], W[b + "norm1.b"])
-        qkv = ops.linear(h, W[b + "qkv.w"], bias=W[b + "qkv.b"]).view(n, L, 3 * d)
-        a = ops.attention_d64(qkv[:, :, :d], qkv[:, :, d:2 * d], qkv[:, :, 2 * d:], self.num_heads)
-        x2 = ops.linear(a.view(n * L, d), W[b + "proj.w"], bias=W[b + "proj.b"], residual=x2)
-        h = ops.layer_norm(x2, W[b + "norm2.g"], W[b + "norm2.b"])
-        h = ops.linear_gelu_rowbias(h, W[b + "fc1.w"], bias=W[b + "fc1.b"])
-        return ops.linear(h, W[b + "fc2.w"], bias=W[b + "fc2.b"], residual=x2).view(n, L, d)
 
     @staticmethod
     def _readout(x, W, s, hp, wp):

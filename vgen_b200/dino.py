@@ -7,9 +7,10 @@ Same constructor arguments and state-dict names, so `dino_deitsmall16_pretrain.p
   patch embedding (conv p x p, stride p, with bias) -> [CLS] + pos_embed -> depth x pre-LN blocks (LayerNorm eps of the
   norm_layer, qkv with bias, softmax attention, proj; fc1 -> GELU(erf) -> fc2) -> norm -> class token
 
-and returns fp32 [n, embed_dim].  Every op is a kernel of libvgen_b200.so: im2col + the wgmma tap-GEMM for the patch
-embedding and the linears (bias and residual in the epilogue), LayerNorm, the head_dim-64 flash attention.  Activations
-are fp16 with fp32 accumulation and statistics; the forward is CUDA-graphed per input signature (n, H, W).
+and returns fp32 [n, embed_dim].  The patch embedding and the blocks are the shared ViT trunk (vgen_b200.vit): every op is
+a kernel of libvgen_b200.so, im2col + the wgmma tap-GEMM for the patch embedding and the linears (bias, GELU and residual
+in the epilogue), LayerNorm, the head_dim-64 flash attention.  Activations are fp16 with fp32 accumulation and
+statistics; the forward is CUDA-graphed per input signature (n, H, W).
 
 Not provided: inputs whose patch grid differs from the trained one (interpolate_pos_encoding), get_last_selfattention,
 get_intermediate_layers and DINOHead raise NotImplementedError.  There is no CPU path: a CPU tensor or a CPU-resident
@@ -22,9 +23,13 @@ import functools
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, vit
 from .graph import graphed
 from .params import SpecModule
+from .vit import f16, f32
+
+# the reference's Block: the state-dict prefixes of LN1, qkv, proj, LN2, fc1, fc2 (vit.pack_block)
+_BLOCK = ("norm1.", "attn.qkv.", "attn.proj.", "norm2.", "mlp.fc1.", "mlp.fc2.")
 
 
 def _ln_eps(norm_layer):
@@ -83,24 +88,11 @@ class VisionTransformer(SpecModule):
         if dev.type != "cuda":
             raise ops._l.VgenError("vgen_b200 DINO forward needs the model on a CUDA device (no CPU path exists)")
         sd = self.state_dict()
-        f16 = lambda t: t.detach().to(device=dev, dtype=torch.float16).contiguous()  # noqa: E731
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-        W = {}
-        w = sd["patch_embed.proj.weight"]                                     # [D, c, p, p] -> [D, (ky, kx, c)] K-padded
-        k = w.shape[1] * w.shape[2] * w.shape[3]
-        wp = torch.zeros(w.shape[0], ((k + 63) // 64) * 64)
-        wp[:, :k] = w.detach().float().cpu().permute(0, 2, 3, 1).reshape(w.shape[0], k)
-        W["patch.w"], W["patch.b"] = f16(wp), f32(sd["patch_embed.proj.bias"])
-        W["cls"], W["pos"] = f16(sd["cls_token"].reshape(1, -1)), f32(sd["pos_embed"].reshape(-1))
+        W = {"patch.w": vit.pack_patch(sd["patch_embed.proj.weight"], dev), "patch.b": f32(sd["patch_embed.proj.bias"], dev),
+             "cls": f16(sd["cls_token"].reshape(1, -1), dev), "pos": f32(sd["pos_embed"].reshape(-1), dev)}
         for i in range(self.depth):
-            p = f"blocks.{i}."
-            for nm in ("norm1.", "norm2."):
-                W[p + nm + "g"], W[p + nm + "b"] = f32(sd[p + nm + "weight"]), f32(sd[p + nm + "bias"])
-            W[p + "qkv.w"] = f16(sd[p + "attn.qkv.weight"])
-            W[p + "qkv.b"] = f32(sd[p + "attn.qkv.bias"]) if self.qkv_bias else None
-            for nm, src in (("proj.", "attn.proj."), ("fc1.", "mlp.fc1."), ("fc2.", "mlp.fc2.")):
-                W[p + nm + "w"], W[p + nm + "b"] = f16(sd[p + src + "weight"]), f32(sd[p + src + "bias"])
-        W["norm.g"], W["norm.b"] = f32(sd["norm.weight"]), f32(sd["norm.bias"])
+            vit.pack_block(W, sd, f"blocks.{i}.", _BLOCK, dev)
+        W["norm.g"], W["norm.b"] = f32(sd["norm.weight"], dev), f32(sd["norm.bias"], dev)
         self._packed = W
         return W
 
@@ -142,28 +134,11 @@ class VisionTransformer(SpecModule):
 
     def _tower(self, img):
         W = self._packed
-        n, H, Wd, _ = img.shape
-        p, D, eps = self.patch_size, self.embed_dim, self.eps
-        gh, gw = H // p, Wd // p
-        col = ops.im2col(img, p, p, p, 0, 0, gh, gw, W["patch.w"].shape[1])
-        patches = ops.linear(col, W["patch.w"], bias=W["patch.b"])
-        L = gh * gw + 1
-        x = torch.empty(n, L, D, device=img.device, dtype=torch.float16)
-        xr = x.view(n, L * D)
-        ops.copy2d(W["cls"].expand(n, D), xr[:, :D])
-        ops.copy2d(patches.view(n, gh * gw * D), xr[:, D:])
-        ops.add_rows_f32_(x, W["pos"])
-        x2 = x.view(n * L, D)
+        x = vit.embed(img, self.patch_size, W["patch.w"], W["patch.b"], W["cls"], W["pos"])
         for i in range(self.depth):
-            q = f"blocks.{i}."
-            h = ops.layer_norm(x2, W[q + "norm1.g"], W[q + "norm1.b"], eps)
-            qkv = ops.linear(h, W[q + "qkv.w"], bias=W[q + "qkv.b"]).view(n, L, 3 * D)
-            a = ops.attention_d64(qkv[:, :, :D], qkv[:, :, D:2 * D], qkv[:, :, 2 * D:], self.num_heads, scale=self.scale)
-            x2 = ops.linear(a.view(n * L, D), W[q + "proj.w"], bias=W[q + "proj.b"], residual=x2)
-            h = ops.layer_norm(x2, W[q + "norm2.g"], W[q + "norm2.b"], eps)
-            h = ops.eltwise("gelu", ops.linear(h, W[q + "fc1.w"], bias=W[q + "fc1.b"]))
-            x2 = ops.linear(h, W[q + "fc2.w"], bias=W[q + "fc2.b"], residual=x2)
-        y = ops.layer_norm(x2.view(n, L * D)[:, :D], W["norm.g"], W["norm.b"], eps)     # the class tokens
+            x = vit.block(x, W, f"blocks.{i}.", self.num_heads, self.eps, attention="d64", scale=self.scale)
+        n, L, D = x.shape
+        y = ops.layer_norm(x.view(n, L * D)[:, :D], W["norm.g"], W["norm.b"], self.eps)     # the class tokens
         return ops.pc_to_cp(y.view(n, 1, D), n, D, 1, torch.float32).view(n, D)
 
     # ---- not provided ---------------------------------------------------------------------------
