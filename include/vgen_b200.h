@@ -250,6 +250,28 @@ int vgen_resize_bicubic_crop_normalize(const uint8_t* src, int64_t n, int64_t h,
 int vgen_video_scores(const float* clip_frames, int64_t f, int64_t e, const float* text, const float* clip_targets,
                       int64_t t, const float* dino_frames, const float* dino_targets, int64_t d, float* out4, void* stream);
 
+/* ---- InstructVideo's segmental video reward (reward.cu) ------------------------------------------------------------ */
+/* The HPSv2 image tower's input of n selected frames.  Output frame i reads source frame frame_idx[i] = v * frames_per + t
+ * at element offset v * s_video + t * s_frame, channel / row / column strides s_c / s_y / s_x (fp32 [b][3][f][h][w] decoder
+ * output, fp32 [n][3][h][w], or uint8 RGB [n][h][w][3] with src_u8 = 1).  Per sample: x * 0.5 + 0.5 (fp32) or x / 255
+ * (uint8), clamp(0, 1); then a separable resize with host-computed taps (hbounds [ow][2] = (first source column, taps),
+ * hcoef fp32 [ow][kh]; vbounds / vcoef the same for rows; source indices past the edge are clamped): F.interpolate's
+ * bilinear, align_corners=False, with or without antialias; then (x - mean[c]) / std[c].  tile_rows: the most source
+ * rows the vertical windows of 16 consecutive output rows span.
+ * out: fp16 channels-last [n][oh][ow][3] (out_f32 = 0, the image tower's input) or fp32 [n][3][oh][ow] (out_f32 = 1).
+ * replaces: reward.py:134-165 (decode output -> mul/add/clamp -> Resize(224) -> Normalize -> frame selection) */
+int vgen_reward_frames(const void* src, int src_u8, const int32_t* frame_idx, int64_t n, int64_t frames_per,
+                       int64_t s_video, int64_t s_frame, int64_t s_c, int64_t s_y, int64_t s_x, int64_t h, int64_t w,
+                       const int32_t* hbounds, const float* hcoef, int64_t kh, const int32_t* vbounds, const float* vcoef,
+                       int64_t kv, int64_t oh, int64_t ow, int64_t tile_rows, const float* mean3, const float* std3,
+                       void* out, int out_f32, void* stream);
+/* reward_scores fp32 [b] of b videos from fp32 image_features [b * s][e] (video-major) and text_features [b][e]:
+ * mean over the s segments of <img / max(||img||, 1e-12), txt / max(||txt||, 1e-12)>, each term times
+ * exp(-|frame_idx[k * s + j] - f / 2| * lambda_tar) when tar != 0 (frame_idx int32 [b * s], may be null without tar).
+ * One block per video.  replaces: reward.py:174-192 */
+int vgen_segment_reward(const float* image_features, const float* text_features, const int32_t* frame_idx, int64_t b,
+                        int64_t s, int64_t e, int64_t f, int tar, float lambda_tar, float* out, void* stream);
+
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */
 int vgen_vae_sample(const void* moments, const float* noise, float* z, int64_t n, int64_t zc, int64_t p, float scale,

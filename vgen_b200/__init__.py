@@ -6,7 +6,8 @@ the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`) and sketch ann
 `SketchSimplification` / `sketch_simplification_gan`), and DreamVideo's textual-inversion text path
 (`FrozenOpenCLIPCustomEmbedder` + `EmbeddingManager`, EMBEDDER / EMBEDMANAGER) with DDIM inversion
 (`DiffusionDDIM.ddim_reverse_sample_loop`), and DreamVideo's evaluation metric (`calculate_metric`, `score_video`,
-`load_clip`, `dino_transform`, with the DINO ViT `vit_small`).
+`load_clip`, `dino_transform`, with the DINO ViT `vit_small`), and InstructVideo's segmental HPSv2 reward
+(`SegmentalReward`, `load_hps`, `segment_indices`).
 
 Every op of the path is a hand-written CUDA kernel in libvgen_b200.so (include/vgen_b200.h); this
 package holds only the host-side mirror of the reference interface.  There is no CPU / PyTorch
@@ -45,6 +46,9 @@ def __getattr__(name):  # lazy: importing the package must not require torch.cud
     if name in ("calculate_metric", "score_video", "load_clip", "dino_transform"):
         from . import metric
         return getattr(metric, name)
+    if name in ("SegmentalReward", "load_hps", "segment_indices"):
+        from . import reward
+        return getattr(reward, name)
     if name in ("vit_tiny", "vit_small", "vit_base"):
         from . import dino
         return getattr(dino, name)

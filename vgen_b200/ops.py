@@ -1004,3 +1004,69 @@ def video_scores(clip_frames, text, clip_targets, dino_frames, dino_targets):
                                      _p(dino_targets) if t else None, d, _p(out), _stream())
     _l.check(rc, "vgen_video_scores")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# InstructVideo's segmental video reward (reward.cu)
+def reward_frames(src, frame_idx, plan, out_f32=False, out=None):
+    """The reward's image-tower input of the frames frame_idx (int32 CUDA [n], flat frame numbers v * f + t) of src:
+    fp32 decoder output [b, 3, f, H, W] or [n, 3, H, W] (any element strides; x * 0.5 + 0.5) or uint8 RGB [n, H, W, 3]
+    (x / 255); clamp(0, 1), the bilinear resize of `plan` (reward.BilinearPlan) and its normalisation -> fp16
+    [n, oh, ow, 3] or, with out_f32, fp32 [n, 3, oh, ow] (into `out` if given)."""
+    if not src.is_cuda or src.dtype not in (torch.float32, torch.uint8):
+        raise _l.VgenError("reward_frames: src must be a CUDA fp32 or uint8 tensor")
+    if src.dtype == torch.uint8:
+        if src.dim() != 4 or src.shape[3] != 3:
+            raise _l.VgenError(f"reward_frames: uint8 frames must be [n, H, W, 3], got {tuple(src.shape)}")
+        nsrc, fp, (h, w) = src.shape[0], 1, src.shape[1:3]
+        sv, sf, sc, sy, sx = src.stride(0), 0, src.stride(3), src.stride(1), src.stride(2)
+    elif src.dim() == 5 and src.shape[1] == 3:
+        nsrc, fp, (h, w) = src.shape[0] * src.shape[2], src.shape[2], src.shape[3:]
+        sv, sc, sf, sy, sx = src.stride()
+    elif src.dim() == 4 and src.shape[1] == 3:
+        nsrc, fp, (h, w) = src.shape[0], 1, src.shape[2:]
+        sv, sc, sy, sx = src.stride()
+        sf = 0
+    else:
+        raise _l.VgenError(f"reward_frames: fp32 frames must be [b, 3, f, H, W] or [n, 3, H, W], got {tuple(src.shape)}")
+    if (h, w) != (plan.h, plan.w):
+        raise _l.VgenError(f"reward_frames: the plan is for {plan.h}x{plan.w} frames, got {h}x{w}")
+    if (frame_idx.dtype != torch.int32 or not frame_idx.is_contiguous() or frame_idx.dim() != 1
+            or frame_idx.device != src.device):
+        raise _l.VgenError(f"reward_frames: frame_idx must be a contiguous int32 [n] tensor on {src.device}")
+    n = frame_idx.shape[0]
+    hb, hk, vb, vk = plan.tables(src.device)
+    oh, ow = plan.oh, plan.ow
+    shape, dtype = ((n, 3, oh, ow), torch.float32) if out_f32 else ((n, oh, ow, 3), torch.float16)
+    if out is None:
+        out = torch.empty(shape, device=src.device, dtype=dtype)
+    elif tuple(out.shape) != shape or out.dtype != dtype or not out.is_contiguous() or out.device != src.device:
+        raise _l.VgenError(f"reward_frames: out must be a contiguous {dtype} tensor {list(shape)} on {src.device}")
+    m3 = (ctypes.c_float * 3)(*[float(v) for v in plan.mean])
+    s3 = (ctypes.c_float * 3)(*[float(v) for v in plan.std])
+    rc = _run("reward_frames", 0.0, n * 3 * h * w * src.element_size() + out.numel() * out.element_size(),
+              lambda: _l.load().vgen_reward_frames(_p(src), 1 if src.dtype == torch.uint8 else 0, _p(frame_idx), n, fp, sv,
+                                                   sf, sc, sy, sx, h, w, _p(hb), _p(hk), hk.shape[1], _p(vb), _p(vk),
+                                                   vk.shape[1], oh, ow, plan.tile_rows, m3, s3, _p(out),
+                                                   1 if out_f32 else 0, _stream()))
+    _l.check(rc, "vgen_reward_frames")
+    return out
+
+
+def segment_reward(image_features, text_features, frame_idx, f, tar, lambda_tar):
+    """reward_scores fp32 [b] from fp32 image_features [b * s, e] (video-major), text_features [b, e] and the segments'
+    frame indices frame_idx (int32 [b, s] on the device; read only with tar) of f-frame videos."""
+    b, e = text_features.shape
+    s = image_features.shape[0] // max(b, 1)
+    for x, nm, shape in ((image_features, "image_features", (b * s, e)), (text_features, "text_features", (b, e))):
+        if x.dtype != torch.float32 or not x.is_cuda or not x.is_contiguous() or tuple(x.shape) != shape:
+            raise _l.VgenError(f"segment_reward: {nm} must be a contiguous CUDA fp32 tensor {list(shape)}")
+    if (frame_idx.dtype != torch.int32 or not frame_idx.is_contiguous() or tuple(frame_idx.shape) != (b, s)
+            or frame_idx.device != text_features.device):
+        raise _l.VgenError(f"segment_reward: frame_idx must be a contiguous int32 tensor [{b}, {s}] on {text_features.device}")
+    out = torch.empty(b, device=text_features.device, dtype=torch.float32)
+    rc = _run("segment_reward", 6.0 * b * s * e, 4.0 * (b * s * e + b * e),
+              lambda: _l.load().vgen_segment_reward(_p(image_features), _p(text_features), _p(frame_idx), b, s, e, int(f),
+                                                    1 if tar else 0, float(lambda_tar), _p(out), _stream()))
+    _l.check(rc, "vgen_segment_reward")
+    return out
