@@ -272,6 +272,23 @@ int vgen_reward_frames(const void* src, int src_u8, const int32_t* frame_idx, in
 int vgen_segment_reward(const float* image_features, const float* text_features, const int32_t* frame_idx, int64_t b,
                         int64_t s, int64_t e, int64_t f, int tar, float lambda_tar, float* out, void* stream);
 
+/* ---- the VideoComposer canny annotator (canny.cu) ------------------------------------------------------------------ */
+/* cv2.Canny edge maps of n frames of c = 1 or 3 channels, h x w, read at element offset i * s_n + ch * s_c + y * s_y +
+ * x * s_x: fp32 in [0, 1] (src_u8 = 0; the bytes are convertScaleAbs(x * 255): |.|, round to nearest even, saturate) or
+ * uint8 (src_u8 = 1; taken as they are).  Thresholds per frame, from the exact median m of its h * w * c bytes (float64):
+ * mode 0 (low, high) as given; mode 1 (1 - 0.33) * m and (1 + 0.33) * m, truncated, high capped at 255; mode 2
+ * trunc((1 - rand[i]) * m) and twice that (rand: fp64 [n] on the device).  Then, as cv2.Canny: swapped if low > high,
+ * floored; 3x3 Sobel with replicated borders, the channel with the largest |dx| + |dy|, the L1 magnitude,
+ * non-maximum suppression, candidates m > low and strong pixels m > high, and hysteresis: a candidate is an edge when it
+ * is 8-connected through candidates to a strong pixel (union-find; the launch count does not depend on the image).
+ * Workspaces: bytes uint8 [n][c][h][w], hist int32 [n][256] (zeroed by the call), thr int32 [n][2] (receives the integer
+ * low, high), cls uint8 [n][h][w], label int32 [n][h][w], keep uint8 [n][h][w].  out: fp32 [n][h][w] of 0.0 / 1.0 (the
+ * condition layout [b][1][f][h][w] for n = b * f).
+ * replaces: tools/annotator/canny/__init__.py:23-48 (convertScaleAbs, np.median, cv2.Canny per frame on the host) */
+int vgen_canny(const void* src, int src_u8, int64_t n, int64_t c, int64_t h, int64_t w, int64_t s_n, int64_t s_c,
+               int64_t s_y, int64_t s_x, int mode, const double* rand, double low, double high, uint8_t* bytes,
+               int32_t* hist, int32_t* thr, uint8_t* cls, int32_t* label, uint8_t* keep, float* out, void* stream);
+
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */
 int vgen_vae_sample(const void* moments, const float* noise, float* z, int64_t n, int64_t zc, int64_t p, float scale,

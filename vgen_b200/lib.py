@@ -36,7 +36,7 @@ class Epilogue(ctypes.Structure):
 
 _lib = None
 
-_vp, _i64, _i32, _f32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_float
+_vp, _i64, _i32, _f32, _f64 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_float, ctypes.c_double
 _EP = ctypes.POINTER(Epilogue)
 
 # name -> argtypes (restype is int unless listed in _RESTYPES); mirrors include/vgen_b200.h 1:1.
@@ -98,6 +98,8 @@ _SIGNATURES = {
     "vgen_reward_frames": [_vp, _i32, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp,
                            _i64, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp],
     "vgen_segment_reward": [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _f32, _vp, _vp],
+    "vgen_canny": [_vp, _i32, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _vp, _f64, _f64, _vp, _vp, _vp, _vp,
+                   _vp, _vp, _vp, _vp],
 }
 _RESTYPES = {"vgen_last_error": ctypes.c_char_p, "vgen_launch_count": ctypes.c_int64,
              "vgen_group_norm_workspace_bytes": ctypes.c_int64}

@@ -1070,3 +1070,41 @@ def segment_reward(image_features, text_features, frame_idx, f, tar, lambda_tar)
                                                     1 if tar else 0, float(lambda_tar), _p(out), _stream()))
     _l.check(rc, "vgen_segment_reward")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# the VideoComposer canny annotator (canny.cu)
+def canny(frames, mode, rand=None, low=0.0, high=0.0, out=None, thresholds=False):
+    """cv2.Canny edge maps (aperture 3, L1 gradient) of frames [n, c, h, w] (any element strides, c = 1 or 3): CUDA fp32
+    in [0, 1], quantised as convertScaleAbs(x * 255), or uint8.  Thresholds from each frame's median: mode 0 (low,
+    high) as given, mode 1 (1 -/+ 0.33) * median, mode 2 (1 - rand[i]) * median and twice that (rand: CUDA fp64 [n]).
+    Returns fp32 [n, h, w] of 0.0 / 1.0 (into `out`, any contiguous tensor of n * h * w fp32, if given) and, with
+    thresholds, also the int32 [n, 2] (low, high) the magnitudes were compared with."""
+    if not frames.is_cuda or frames.dtype not in (torch.float32, torch.uint8):
+        raise _l.VgenError(f"canny: frames must be a CUDA fp32 or uint8 tensor, got {frames.dtype} on {frames.device}")
+    if frames.dim() != 4 or frames.shape[1] not in (1, 3) or frames.shape[2] == 0 or frames.shape[3] == 0:
+        raise _l.VgenError(f"canny: frames must be [n, c, h, w] with c = 1 or 3, got {tuple(frames.shape)}")
+    n, c, h, w = frames.shape
+    dev = frames.device
+    if mode == 2:
+        if (rand is None or rand.dtype != torch.float64 or rand.device != dev or not rand.is_contiguous()
+                or tuple(rand.shape) != (n,)):
+            raise _l.VgenError(f"canny: rand must be a contiguous fp64 tensor [{n}] on {dev}")
+    elif mode not in (0, 1):
+        raise _l.VgenError(f"canny: mode must be 0, 1 or 2, got {mode}")
+    if out is None:
+        out = torch.empty(n, h, w, device=dev, dtype=torch.float32)
+    elif out.numel() != n * h * w or out.dtype != torch.float32 or not out.is_contiguous() or out.device != dev:
+        raise _l.VgenError(f"canny: out must be a contiguous fp32 tensor of {n * h * w} elements on {dev}")
+    u8 = lambda *s: torch.empty(s, device=dev, dtype=torch.uint8)  # noqa: E731
+    i32 = lambda *s: torch.empty(s, device=dev, dtype=torch.int32)  # noqa: E731
+    bytes_, hist, thr, cls, label, keep = u8(n, c, h, w), i32(n, 256), i32(n, 2), u8(n, h, w), i32(n, h, w), u8(n, h, w)
+    s_n, s_c, s_y, s_x = frames.stride()
+    px = n * h * w
+    rc = _run("canny", 0.0, n * c * h * w * (frames.element_size() + 2) + px * 16,
+              lambda: _l.load().vgen_canny(_p(frames), 1 if frames.dtype == torch.uint8 else 0, n, c, h, w, s_n, s_c, s_y,
+                                           s_x, mode, _p(rand) if mode == 2 else None, float(low), float(high),
+                                           _p(bytes_), _p(hist), _p(thr), _p(cls), _p(label), _p(keep), _p(out),
+                                           _stream()))
+    _l.check(rc, "vgen_canny")
+    return (out, thr) if thresholds else out
