@@ -104,6 +104,19 @@ int vgen_tconv3(const void* x, int64_t f, int64_t hw, int64_t c, const void* w, 
 int vgen_tconv3_batch(const void* x, int64_t batch, int64_t f, int64_t hw, int64_t c, const void* w, int64_t n,
                       void* out, int64_t ldo, const vgen_epilogue* epi, void* stream);
 
+/* ---- FP8 (e4m3) linear (tapgemm_fp8_sm90.cu; opt-in, UNet fp8_linear=True) ------------------------------------- */
+/* Row quantiser: x fp16 [m][k] (row stride ldx) -> q e4m3 codes [m][k] (row stride ldq, bytes) and fp32 scale[m] =
+ * amax_row / 448, q = e4m3_satfinite(x / scale) rounded to nearest even; an all-zero row gets scale 1.
+ * k, ldx, ldq multiples of 8; x 16-byte and q 8-byte aligned. */
+int vgen_quantize_rows_e4m3(const void* x, int64_t m, int64_t k, int64_t ldx, void* q, int64_t ldq, float* scale,
+                            void* stream);
+/* out[m][n] = epi(a_scale[m] * w_scale[n] * (a[m][:k] . w[n][:k]))  with e4m3 a (row stride lda bytes) and w [n][k],
+ * fp32 accumulation promoted out of the tensor core every 128 K.  epi: alpha, bias, residual, GEGLU and bn (64 or 128;
+ * 0 = auto) as for vgen_linear; no group_bias / folded LayerNorm.  k and lda multiples of 16, a / w 16-byte aligned.
+ * replaces (opt-in, changes the numerics): the transformer projections of vgen_linear, util.py:224-229,338,353,711,736 */
+int vgen_linear_fp8(const void* a, const float* a_scale, int64_t m, int64_t k, int64_t lda, const void* w,
+                    const float* w_scale, int64_t n, void* out, int64_t ldo, const vgen_epilogue* epi, void* stream);
+
 /* ---- normalisation (norm.cu; HBM-bound, fp32 statistics) ---------------------------------------- */
 /* GroupNorm(32 groups) over x[n][p][c] fp16 (statistics per sample n over p*c/32 values), optional
  * SiLU, y fp16.  For the 5-D (all-frames-jointly) norms pass n = batch, p = f*h*w.

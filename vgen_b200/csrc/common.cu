@@ -61,8 +61,21 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
+static int make_tmap(CUtensorMapDataType dtype, CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes);
+
 int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                   const uint32_t* box, int swizzle_bytes) {
+  return make_tmap(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, map, base, rank, dims, strides_bytes, box, swizzle_bytes);
+}
+
+int make_tmap_u8(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box, int swizzle_bytes) {
+  return make_tmap(CU_TENSOR_MAP_DATA_TYPE_UINT8, map, base, rank, dims, strides_bytes, box, swizzle_bytes);
+}
+
+static int make_tmap(CUtensorMapDataType dtype, CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return fail("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
   cuuint64_t gdim[5];
@@ -78,7 +91,7 @@ int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* 
     gstr[i] = strides_bytes[i];
     if (gstr[i] % 16 != 0) return fail("tensor map: strides must be multiples of 16 bytes");
   }
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim,
+  CUresult r = enc(map, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim,
                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,

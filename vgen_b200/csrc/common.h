@@ -38,6 +38,9 @@ int check_cuda(cudaError_t e, const char* what);
 // strides_bytes has rank-1 entries (dims 1..rank-1). Out-of-bounds elements read as zero / are not written.
 int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                   const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128);
+// Same for a tensor of bytes (e4m3 codes): dims / box in elements = bytes.
+int make_tmap_u8(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128);
 
 int sm_count();            // of the CURRENT device (cached per device)
 int current_device();

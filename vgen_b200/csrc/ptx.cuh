@@ -217,6 +217,22 @@ VG_WGMMA_SS(256, VG_PH_0 VG_PH_1 VG_PH_2 VG_PH_3 VG_PH_4 VG_PH_5 VG_PH_6 VG_PH_7
             VG_D16(32), VG_D16(48), VG_D16(64), VG_D16(80), VG_D16(96), VG_D16(112))
 #undef VG_WGMMA_SS
 
+// D[64 x N, fp32 registers] (+)= A[64 x 32, smem] * B[N x 32, smem]^T, e4m3 operands, both K-major (the only operand
+// layout wgmma takes for 8-bit types).  Same fragment layout as wgmma_ss; one instruction covers K = 32 (32 bytes).
+template <int N>
+__device__ __forceinline__ void wgmma_ss_e4m3(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, int accumulate);
+#define VG_WGMMA_SS_E4M3(N, PH, A, B, S, ...)                                                                           \
+  template <>                                                                                                          \
+  __device__ __forceinline__ void wgmma_ss_e4m3<N>(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, int accumulate) { \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #S ", 0;\n\t"                                              \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k32.f32.e4m3.e4m3 {" PH "}, %" #A ", %" #B ", p, 1, 1;\n\t}"  \
+                 : __VA_ARGS__                                                                                         \
+                 : "l"(a_desc), "l"(b_desc), "r"(accumulate));                                                         \
+  }
+VG_WGMMA_SS_E4M3(64, VG_PH_0 VG_PH_1, 32, 33, 34, VG_D16(0), VG_D16(16))
+VG_WGMMA_SS_E4M3(128, VG_PH_0 VG_PH_1 VG_PH_2 VG_PH_3, 64, 65, 66, VG_D16(0), VG_D16(16), VG_D16(32), VG_D16(48))
+#undef VG_WGMMA_SS_E4M3
+
 // D[64 x 64] (+)= A[64 x 16, registers] * B[16 x 64, smem, MN-major]: the P V product of the attention kernels.
 // a[0..3]: the m16k16 fragment of this thread's warp -- {row g, k 2q..2q+1}, {row g+8, same k}, {row g, k 2q+8..2q+9},
 // {row g+8, same k} -- which is what two adjacent 8-column groups of a wgmma accumulator hold once packed to fp16.

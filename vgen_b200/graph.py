@@ -35,6 +35,12 @@ def enabled() -> bool:
     return os.environ.get("VGEN_CUDA_GRAPH", "1") != "0"
 
 
+def _mode(owner):
+    """The module's numerics mode, part of every graph signature: a graph captured with one fp8_linear setting is never
+    replayed under the other (re-packing drops the graphs as well; this keeps the key honest on its own)."""
+    return (("fp8_linear", bool(getattr(owner, "fp8_linear", False))),)
+
+
 class _Entry:
     __slots__ = ("graph", "static", "out", "uses")
 
@@ -80,6 +86,7 @@ class GraphCache:
         if flat is None:
             return fn(owner, *args, **kwargs)
         tensors, sig, rebuild = flat
+        sig = _mode(owner) + sig
         ent = self.entries.get(sig)
         if ent is None:
             n = self.seen.get(sig, 0)
@@ -129,7 +136,8 @@ def graphed(fn):
                 flat = GraphCache._flatten(args, kwargs)
                 if flat is not None:
                     c = self._packed.setdefault("__graphs__", {}).setdefault(fn.__name__, GraphCache())
-                    c.seen[flat[1]] = max(c.seen.get(flat[1], 0), 1)
+                    key = _mode(self) + flat[1]
+                    c.seen[key] = max(c.seen.get(key, 0), 1)
             return out
         if (not enabled() or ops.PROF is not None or not getattr(self, "use_cuda_graph", True)
                 or torch.cuda.is_current_stream_capturing()):

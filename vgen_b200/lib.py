@@ -51,6 +51,8 @@ _SIGNATURES = {
     "vgen_conv2d_3x3": [_vp, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _EP, _vp],
     "vgen_tconv3": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _EP, _vp],
     "vgen_tconv3_batch": [_vp, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _EP, _vp],
+    "vgen_quantize_rows_e4m3": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp],
+    "vgen_linear_fp8": [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _i64, _EP, _vp],
     "vgen_group_norm_workspace_bytes": [_i64],
     "vgen_group_norm": [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _f32, _i32, _vp, _vp],
     "vgen_layer_norm": [_vp, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _f32, _vp],

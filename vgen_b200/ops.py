@@ -147,6 +147,79 @@ def linear(a, w, bias=None, residual=None, alpha=1.0, geglu=False, out=None, bn=
     return out
 
 
+E4M3_MAX = 448.0
+
+
+def quantize_weight_e4m3(w):
+    """Per-output-channel e4m3 quantisation of a GEMM weight [n, k] (any float dtype; the amax is taken in fp32):
+    -> (codes uint8 [n, k], scale fp32 [n]) with scale = amax / 448 (1 for an all-zero row) and
+    codes = e4m3(w / scale), round to nearest even.  Runs on w's device (pack time, not the hot path)."""
+    w = w.detach().float()
+    amax = w.abs().amax(dim=1)
+    scale = torch.where(amax > 0, (amax.double() / E4M3_MAX).float(), torch.ones_like(amax))   # correctly rounded
+    codes = (w / scale[:, None]).to(torch.float8_e4m3fn).view(torch.uint8)
+    return codes.contiguous(), scale.contiguous()
+
+
+def quantize_rows_e4m3(x, out=None, scale=None):
+    """x fp16 [m, k] (a row-strided 2-D view is fine) -> (codes uint8 [m, k], scale fp32 [m]): one launch of the row
+    quantiser, scale = amax_row / 448 (1 for an all-zero row), codes = e4m3(x / scale) with saturation."""
+    _chk16(x, "x")
+    x2, ldx = _rows_view(x, "x")
+    m, k = x2.shape
+    if out is None:
+        out = torch.empty(m, k, device=x.device, dtype=torch.uint8)
+    if scale is None:
+        scale = torch.empty(m, device=x.device, dtype=torch.float32)
+    if out.dtype != torch.uint8 or tuple(out.shape) != (m, k) or out.stride(1) != 1:
+        raise _l.VgenError(f"quantize_rows_e4m3: out must be uint8 [{m}, {k}] with contiguous rows")
+    if scale.dtype != torch.float32 or scale.numel() != m or not scale.is_contiguous():
+        raise _l.VgenError(f"quantize_rows_e4m3: scale must be contiguous fp32 [{m}]")
+    rc = _run("quantize_e4m3", 0.0, 3.0 * m * k,
+              lambda: _l.load().vgen_quantize_rows_e4m3(_p(x2), m, k, ldx, _p(out), out.stride(0), _p(scale), _stream()),
+              tag=f"quantize m{m} k{k}")
+    _l.check(rc, "vgen_quantize_rows_e4m3")
+    return out, scale
+
+
+def linear_e4m3(a8, a_scale, w8, w_scale, bias=None, residual=None, alpha=1.0, geglu=False, out=None, bn=0):
+    """out[m, n] = epi(a_scale[m] * w_scale[n] * (a8[m, k] @ w8[n, k]^T)) on e4m3 codes (uint8 tensors) with fp32
+    accumulation; the epilogue (bias / residual / GEGLU, fp16 output) is that of linear()."""
+    if a8.dtype != torch.uint8 or w8.dtype != torch.uint8 or not a8.is_cuda:
+        raise _l.VgenError("linear_e4m3: a8 and w8 must be CUDA uint8 tensors of e4m3 codes")
+    a2, lda = _rows_view(a8, "a8")
+    m, k = a2.shape
+    n = w8.shape[0]
+    if w8.dim() != 2 or w8.shape[1] != k or not w8.is_contiguous():
+        raise _l.VgenError(f"linear_e4m3: weight {tuple(w8.shape)} does not match k={k}")
+    for t, cnt, name in ((a_scale, m, "a_scale"), (w_scale, n, "w_scale")):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != cnt:
+            raise _l.VgenError(f"linear_e4m3: {name} must be contiguous fp32 [{cnt}]")
+    n_out = n // 2 if geglu else n
+    if out is None:
+        out = torch.empty(*a8.shape[:-1], n_out, device=a8.device, dtype=torch.float16)
+    o2, ldo = _rows_view(out, "out")
+    e, keep = _epilogue(n_out, bias, None, residual, alpha, geglu, bn)
+    rc = _run("tapgemm_fp8", 2.0 * m * n * k, 1.0 * (m * k + n * k) + 2.0 * m * n_out,
+              lambda: _l.load().vgen_linear_fp8(_p(a2), _p(a_scale), m, k, lda, _p(w8), _p(w_scale), n, _p(o2), ldo,
+                                                ctypes.byref(e), _stream()),
+              tag=f"linear_fp8 m{m} k{k} n{n}{' geglu' if geglu else ''}{' res' if residual is not None else ''}")
+    _l.check(rc, "vgen_linear_fp8")
+    return out
+
+
+def linear_fp8(a, w8, w_scale, bias=None, residual=None, alpha=1.0, geglu=False, out=None, bn=0):
+    """linear() with e4m3 operands: the fp16 activations `a` are quantised per row (quantize_rows_e4m3), then multiplied
+    with the per-channel quantised weight (w8, w_scale from quantize_weight_e4m3) by the FP8 tap-GEMM."""
+    lead = a.shape[:-1]
+    a8, a_scale = quantize_rows_e4m3(a)
+    n_out = w8.shape[0] // 2 if geglu else w8.shape[0]
+    if out is None:
+        out = torch.empty(*lead, n_out, device=a.device, dtype=torch.float16)
+    linear_e4m3(a8, a_scale, w8, w_scale, bias=bias, residual=residual, alpha=alpha, geglu=geglu, out=out, bn=bn)
+    return out
+
+
 def linear_gelu_rowbias(a, w, bias=None, row_bias=None, rows_per_group=1, out=None):
     """out[m, j] = fp16(gelu_erf(a[m] . w[j] + bias[j] + row_bias[m // rows_per_group, j])): the adapter down projection.
     The fp32 row bias [groups, n] (a row-strided 2-D view is fine) is added to the fp32 accumulator before the activation;

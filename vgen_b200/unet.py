@@ -55,6 +55,14 @@ def _geglu_bn(n):
     raise ValueError(f"GEGLU width {n} is not a multiple of 64")
 
 
+def _geglu_bn_fp8(n):
+    """GEGLU N tile of the FP8 tap-GEMM (64 or 128)."""
+    for bn in (128, 64):
+        if n % bn == 0:
+            return bn
+    raise ValueError(f"GEGLU width {n} is not a multiple of 64")
+
+
 class _UNetBase(SpecModule):
     KIND = "t2v"
     cfg_batch = True  # samplers may evaluate the cond / uncond CFG branches as one batch-2b forward (diffusion.cfg_forward)
@@ -72,9 +80,10 @@ class _UNetBase(SpecModule):
                  attn_scales=[1 / 2, 1 / 4, 1 / 8], use_scale_shift_norm=True, dropout=0.1, temporal_attn_times=1,
                  temporal_attention=True, use_checkpoint=False, use_image_dataset=False, use_sim_mask=False,
                  training=True, inpainting=True, use_fps_condition=False, p_all_zero=0.1, p_all_keep=0.1, zero_y=None,
-                 adapter_transformer_layers=1, concat_dim=8, context_embedding_depth=4, **kwargs):
+                 adapter_transformer_layers=1, concat_dim=8, context_embedding_depth=4, fp8_linear=False, **kwargs):
         super().__init__()
         self.cfg = config
+        self.fp8_linear = fp8_linear
         if head_dim != 64:
             raise NotImplementedError("vgen_b200: head_dim must be 64 (all released VGen checkpoints)")
         if use_image_dataset:
@@ -104,6 +113,33 @@ class _UNetBase(SpecModule):
     def _plan_kwargs(self, config):
         """Extra unet_plan arguments a subclass reads from `config`."""
         return {}
+
+    # Opt-in FP8 mode (constructor keyword fp8_linear=True): the Linear / k=1 projections of the spatial and temporal
+    # transformer blocks (proj_in, fused q/k/v and the cross-attention q, to_out, the GEGLU projection, the FF down
+    # projection, proj_out) are packed as per-output-channel e4m3 codes + fp32 scales and run on the FP8 tap-GEMM with
+    # per-row quantised activations.  Everything else stays fp16.  It changes the outputs (a precision / speed trade-off);
+    # off, the model is exactly the fp16 one.  Setting the attribute re-packs (and so drops every captured graph).
+    _fp8 = False
+
+    @property
+    def fp8_linear(self):
+        return self._fp8
+
+    @fp8_linear.setter
+    def fp8_linear(self, value):
+        if not isinstance(value, bool):
+            raise ValueError(f"vgen_b200: fp8_linear must be True or False, got {value!r}")
+        if value != self._fp8:
+            self._fp8 = value
+            self.invalidate_packed()
+
+    @staticmethod
+    def _proj(x, W, key, **kw):
+        """ops.linear of the packed projection `key`, or its FP8 form when the pack quantised it (key.e4m3_scale)."""
+        s = W.get(key + ".e4m3_scale")
+        if s is None:
+            return ops.linear(x, W[key], **kw)
+        return ops.linear_fp8(x, W[key], s, **kw)
 
     # ------------------------------------------------------------------------------ weight packing
     def _pack_state_dict(self):
@@ -141,6 +177,10 @@ class _UNetBase(SpecModule):
             norm(e + "0.norm."), lin(e + "0.fn.to_qkv.", bias=False), lin(e + "0.fn.to_out.0.")
             lin(e + "1.net.0.0."), lin(e + "1.net.2.")
 
+        def fp8(key, wmat):
+            """fp8_linear: the projection `key` as e4m3 codes + per-output-channel scales, from the fp32 masters."""
+            W[key], W[key + ".e4m3_scale"] = ops.quantize_weight_e4m3(wmat.detach().to(device=dev, dtype=torch.float32))
+
         def fold(key, wmat, bias, nrm):
             """LayerNorm `nrm` folded into the linear `key` that consumes it (ops.fold_layer_norm)."""
             wf, cs, lb = ops.fold_layer_norm(wmat, bias, sd[nrm + "weight"], sd[nrm + "bias"])
@@ -148,7 +188,8 @@ class _UNetBase(SpecModule):
 
         def block(p, cross, cross1=False):
             a1, a2 = p + "attn1.", p + "attn2."
-            ln_fold = self.FOLD_LN and not cross1
+            q8 = self._fp8 and not cross1   # HiGen's context transformer (cross1) stays fp16 like the other condition paths
+            ln_fold = self.FOLD_LN and not cross1 and not q8
             if cross1:   # disable_self_attn=True: attn1 attends to the context as well (util.py:700-702)
                 W[a1 + "q"] = _f16(sd[a1 + "to_q.weight"], dev)
                 W[a1 + "kv"] = _f16(torch.cat([sd[a1 + "to_k.weight"], sd[a1 + "to_v.weight"]], 0), dev)
@@ -164,7 +205,7 @@ class _UNetBase(SpecModule):
             for nm in ("norm1.", "norm2.", "norm3."):
                 norm(p + nm)
             gw, gb = sd[p + "ff.net.0.proj.weight"].detach().float(), sd[p + "ff.net.0.proj.bias"].detach().float()
-            bn = _geglu_bn(gw.shape[0])
+            bn = _geglu_bn_fp8(gw.shape[0]) if q8 else _geglu_bn(gw.shape[0])
             if ln_fold:
                 # norm1 -> attn1.qkv, norm2 -> attn2.q (cross) / attn2.qkv, norm3 -> GEGLU projection
                 fold(a1 + "qkv", torch.cat([sd[a1 + "to_q.weight"], sd[a1 + "to_k.weight"], sd[a1 + "to_v.weight"]], 0), None, p + "norm1.")
@@ -180,6 +221,15 @@ class _UNetBase(SpecModule):
             if ln_fold:
                 W[p + "ff.geglu.cs"] = _f32(W[p + "ff.geglu.w"].double().sum(1), dev)
             lin(p + "ff.net.2.")
+            if q8:
+                for a in (a1, a2):
+                    if a + "qkv" in W:
+                        fp8(a + "qkv", torch.cat([sd[a + "to_q.weight"], sd[a + "to_k.weight"], sd[a + "to_v.weight"]], 0))
+                    fp8(a + "to_out.0.w", sd[a + "to_out.0.weight"])
+                if cross:
+                    fp8(a2 + "q", sd[a2 + "to_q.weight"])
+                fp8(p + "ff.geglu.w", wp)
+                fp8(p + "ff.net.2.w", sd[p + "ff.net.2.weight"])
 
         cond_w, cond_v = [], []   # conditioned adapters: stacked down.W @ condition_linear.W / down.W @ condition_linear.b
 
@@ -202,6 +252,7 @@ class _UNetBase(SpecModule):
                 ad = {"pos": positions[idx], "hp": hp, "down.w": _f16(wd_p, dev), "down.b": _f32(bd_p, dev), "off": None}
                 if positions[idx] == "parallel":
                     wo = sd[q + out + "weight"].detach().double().cpu()
+                    W.pop(q + out + "w.e4m3_scale", None)   # the projection fused with the adapter's up stays fp16
                     W[q + out + "w"] = _f16(torch.cat([wo, wu_p], dim=1), dev)
                     W[q + out + "b"] = _f32(sd[q + out + "bias"].detach().double().cpu() + bu, dev)
                 else:
@@ -233,6 +284,10 @@ class _UNetBase(SpecModule):
             elif L.kind == "temporal":
                 norm(p + "norm."), lin(p + "proj_in."), block(p + "transformer_blocks.0.", False), lin(p + "proj_out.")
                 adapters(p + "transformer_blocks.0.", self.plan.temporal_adapters, self.plan.temporal_adapter_positions)
+            if self._fp8 and L.kind in ("spatial", "temporal"):
+                for pr in ("proj_in.", "proj_out."):
+                    w = sd[p + pr + "weight"]
+                    fp8(p + pr + "w", w.reshape(w.shape[0], -1))
             elif L.kind == "down":
                 conv3(p + "op.")
             elif L.kind == "up":
@@ -332,7 +387,7 @@ class _UNetBase(SpecModule):
         the weights (key.cs present) only the row statistics are computed and the GEMM epilogue applies them."""
         if key + ".cs" in W:
             return ops.linear(t, W[key], bias=W[key + ".lb"], ln=(ops.row_stats(t), W[key + ".cs"]))
-        return ops.linear(ops.layer_norm(t, W[nrm + "g"], W[nrm + "b"]), W[key])
+        return _UNetBase._proj(ops.layer_norm(t, W[nrm + "g"], W[nrm + "b"]), W, key)
 
     def _self_attn_qkv_spatial(self, t, W, p, nrm, n, hw, inner):
         qkv = self._ln_linear(t, W, p + "qkv", nrm)             # [M, 3*inner]
@@ -347,9 +402,9 @@ class _UNetBase(SpecModule):
         t' = t + sublayer(t).  Without one it is the plain projection with the residual."""
         ad = W.get(p + mod)
         if ad is None:
-            return ops.linear(produce(None).view(-1, width), W[p + out + "w"], bias=W[p + out + "b"], residual=t)
+            return self._proj(produce(None).view(-1, width), W, p + out + "w", bias=W[p + out + "b"], residual=t)
         if ad["pos"] == "serial":
-            t = ops.linear(produce(None).view(-1, width), W[p + out + "w"], bias=W[p + out + "b"], residual=t)
+            t = self._proj(produce(None).view(-1, width), W, p + out + "w", bias=W[p + out + "b"], residual=t)
             h = self._adapter_down(t, ad, hw)
             return ops.linear(h, ad["up.w"], bias=ad["up.b"], residual=t)
         buf = torch.empty(t.shape[0], width + ad["hp"], device=t.device, dtype=torch.float16)
@@ -385,7 +440,7 @@ class _UNetBase(SpecModule):
                 return ops.linear(t, W[p + "ff.geglu.w"], bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"],
                                   ln=(ops.row_stats(t), W[p + "ff.geglu.cs"]), out=out)
             xn = ops.layer_norm(t, W[p + "norm3.g"], W[p + "norm3.b"])
-            return ops.linear(xn, W[p + "ff.geglu.w"], bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"], out=out)
+            return self._proj(xn, W, p + "ff.geglu.w", bias=W[p + "ff.geglu.b"], geglu=True, bn=W[p + "ff.geglu.bn"], out=out)
         return self._sublayer_out(t, W, p, "ff_adapter", "ff.net.2.", W[p + "ff.geglu.w"].shape[0] // 2, hw, geglu)
 
     def _spatial_transformer(self, x, ctx_tokens, L, W, f):
@@ -393,9 +448,9 @@ class _UNetBase(SpecModule):
         p = L.prefix
         n, h, w, c = x.shape
         g = ops.group_norm(x, W[p + "norm.g"], W[p + "norm.b"], 1e-6, False)
-        t = ops.linear(g.view(-1, c), W[p + "proj_in.w"], bias=W[p + "proj_in.b"])
+        t = self._proj(g.view(-1, c), W, p + "proj_in.w", bias=W[p + "proj_in.b"])
         t = self._basic_block_spatial(t, ctx_tokens, W, p + "transformer_blocks.0.", L.heads, n, h * w, L.inner, f)
-        out = ops.linear(t, W[p + "proj_out.w"], bias=W[p + "proj_out.b"], residual=x.view(-1, c))
+        out = self._proj(t, W, p + "proj_out.w", bias=W[p + "proj_out.b"], residual=x.view(-1, c))
         return out.view(n, h, w, c)
 
     def _temporal_attn(self, t, W, p, nrm, heads, b, f, hw, inner, out=None):
@@ -413,13 +468,13 @@ class _UNetBase(SpecModule):
         n, h, w, c = x.shape
         hw, inner = h * w, L.inner
         g = ops.group_norm(x, W[p + "norm.g"], W[p + "norm.b"], 1e-6, False, n=b)
-        t = ops.linear(g.view(-1, c), W[p + "proj_in.w"], bias=W[p + "proj_in.b"])
+        t = self._proj(g.view(-1, c), W, p + "proj_in.w", bias=W[p + "proj_in.b"])
         q = p + "transformer_blocks.0."
         for att, nrm, mod in (("attn1.", "norm1.", "attn_adapter"), ("attn2.", "norm2.", "cross_attn_adapter")):
             t = self._sublayer_out(t, W, q, mod, att + "to_out.0.", inner, hw, lambda o, t=t, att=att, nrm=nrm: self._temporal_attn(
                 t, W, q + att, q + nrm, L.heads, b, f, hw, inner, out=o))
         t = self._feed_forward(t, W, q, hw)
-        out = ops.linear(t, W[p + "proj_out.w"], bias=W[p + "proj_out.b"], residual=x.view(-1, c))
+        out = self._proj(t, W, p + "proj_out.w", bias=W[p + "proj_out.b"], residual=x.view(-1, c))
         return out.view(n, h, w, c)
 
     def _run_layer(self, x, L, W, emb, ctx_tokens, b, f, conv_in_residual=None):
