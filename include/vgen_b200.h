@@ -35,6 +35,10 @@ int64_t vgen_launch_count(void);
 /* tap-GEMM implementation: 0 = auto (default: the wgmma kernel whenever the channel count is a multiple of 64, the SIMT
  * kernel otherwise), 1 = SIMT cross-check kernel everywhere (debug). */
 int vgen_set_tapgemm_impl(int impl);
+/* tap-GEMM N tile: 0 = heuristic (default); 32..256 in steps of 32 = that tile for every fp16 tap-GEMM launch whose
+ * epilogue leaves bn at 0, including vgen_linear_gelu_rowbias (debug: tests reach each kernel instantiation with it).
+ * A tile the launch cannot use (GEGLU: bn % 64 != 0 or n % bn != 0; GELU / row bias: bn > 224) fails that launch. */
+int vgen_set_tapgemm_bn(int bn);
 
 /* ---- tap-GEMM family (wgmma + TMA; tapgemm_sm90.cu) -------------------------------------------- */
 typedef struct vgen_epilogue {
@@ -43,9 +47,10 @@ typedef struct vgen_epilogue {
   const void* group_bias;   /* fp16 [groups][n] or NULL: per-frame bias, added after fp16 rounding     */
   int64_t group_bias_ld;    /*   (ResBlock "h + emb_out": tools/modules/unet/util.py:909-919)          */
   int64_t group_bias_div;   /*   row = image_index / group_bias_div (frames per video); 0 or 1 = per image */
-  const void* residual;     /* fp16 [rows][n] or NULL: added after fp16 rounding (skip / x_in adds)    */
-  int64_t residual_ld;
-  int geglu;                /* 1: out[rows][n/2] = value * gelu(gate); W rows interleaved per bn block */
+  const void* residual;     /* fp16 [rows][n] or NULL: added after fp16 rounding (skip / x_in adds);  */
+  int64_t residual_ld;      /*   not with geglu                                                       */
+  int geglu;                /* 1: out[rows][n/2] = value * gelu(gate); W rows interleaved per bn block; */
+                            /*   bias 16-byte aligned, no residual / group_bias                       */
   int bn;                   /* N tile (32..256, multiple of 32; GEGLU: multiple of 64); 0 = auto       */
   /* LayerNorm folded into the GEMM (vgen_linear only): with w = W * diag(gamma) (rounded to fp16), col_sum[n] =
    * sum_k w[n][k], bias = b + W beta and row_stats[r] = {rstd_r, -mean_r * rstd_r} (vgen_row_stats),
@@ -111,8 +116,9 @@ int vgen_tconv3_batch(const void* x, int64_t batch, int64_t f, int64_t hw, int64
 int vgen_quantize_rows_e4m3(const void* x, int64_t m, int64_t k, int64_t ldx, void* q, int64_t ldq, float* scale,
                             void* stream);
 /* out[m][n] = epi(a_scale[m] * w_scale[n] * (a[m][:k] . w[n][:k]))  with e4m3 a (row stride lda bytes) and w [n][k],
- * fp32 accumulation promoted out of the tensor core every 128 K.  epi: alpha, bias, residual, GEGLU and bn (64 or 128;
- * 0 = auto) as for vgen_linear; no group_bias / folded LayerNorm.  k and lda multiples of 16, a / w 16-byte aligned.
+ * fp32 accumulation promoted out of the tensor core every 128 K.  epi: alpha, bias, and either a residual or GEGLU (not
+ * both; GEGLU needs a 16-byte aligned bias), and bn (64 or 128; 0 = auto) as for vgen_linear; no group_bias / folded
+ * LayerNorm.  k and lda multiples of 16, a / w 16-byte aligned.
  * replaces (opt-in, changes the numerics): the transformer projections of vgen_linear, util.py:224-229,338,353,711,736 */
 int vgen_linear_fp8(const void* a, const float* a_scale, int64_t m, int64_t k, int64_t lda, const void* w,
                     const float* w_scale, int64_t n, void* out, int64_t ldo, const vgen_epilogue* epi, void* stream);

@@ -169,6 +169,9 @@ def test_library_exports_every_declared_symbol():
         assert launched == 0
     assert l.vgen_set_tapgemm_impl(7) != 0 and b"impl" in l.vgen_last_error()
     assert l.vgen_set_tapgemm_impl(0) == 0
+    for bad in (-32, 16, 48, 288):
+        assert l.vgen_set_tapgemm_bn(bad) != 0 and b"bn must be" in l.vgen_last_error()
+    assert l.vgen_set_tapgemm_bn(96) == 0 and l.vgen_set_tapgemm_bn(0) == 0
     assert l.vgen_group_norm_workspace_bytes(2) > 0
     assert ctypes.sizeof(lib.Epilogue) == 80       # struct vgen_epilogue layout (x86-64 SysV; ABI 2 added row_stats, col_sum)
 

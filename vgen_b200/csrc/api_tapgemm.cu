@@ -8,6 +8,7 @@
 namespace vg {
 
 static int g_tapgemm_impl = 0;  // 0 = auto (wgmma whenever C % 64 == 0, else simt), 1 = simt
+static int g_tapgemm_bn = 0;    // 0 = pick_bn; else the N tile of every launch whose epilogue leaves bn at 0 (debug)
 
 // N tile.  With many M tiles the cost is the padded N extent plus a per-tile constant (~24 columns' worth of
 // epilogue / pipeline fill).  With FEW M tiles (the coarse levels of the UNet) the persistent grid runs
@@ -71,6 +72,8 @@ static int fill_epilogue(TapGemmArgs* t, void* out, long ldo, const vgen_epilogu
   e.residual = epi ? reinterpret_cast<const __half*>(epi->residual) : nullptr;
   e.ldr = epi ? epi->residual_ld : 0;
   e.geglu = epi ? epi->geglu : 0;
+  // the GEGLU epilogue (wgmma and SIMT alike) computes value * gelu(gate) and nothing after it
+  VG_REQUIRE(!e.geglu || (!e.residual && !e.group_bias), "tapgemm: the GEGLU epilogue takes no residual or per-frame bias");
   e.row_stats = epi ? reinterpret_cast<const float2*>(epi->row_stats) : nullptr;
   e.col_sum = epi ? epi->col_sum : nullptr;
   VG_REQUIRE((e.row_stats == nullptr) == (e.col_sum == nullptr), "tapgemm: row_stats and col_sum go together");
@@ -89,7 +92,9 @@ static int finish_and_launch(TapGemmArgs* t, const vgen_epilogue* epi, void* str
   TapGemmShape& s = t->shape;
   s.kc = s.c / 64;
   const long m_tiles_all = (long)s.d3 * cdiv(s.d2, s.box2) * cdiv(s.d1, s.box1);
-  int bn = (epi && epi->bn > 0) ? epi->bn : pick_bn(s.n, t->epi.geglu, m_tiles_all, sm_count(), t->epi.gelu ? kMaxBnGelu : 256);
+  int bn = (epi && epi->bn > 0) ? epi->bn
+           : g_tapgemm_bn > 0   ? g_tapgemm_bn
+                                : pick_bn(s.n, t->epi.geglu, m_tiles_all, sm_count(), t->epi.gelu ? kMaxBnGelu : 256);
   VG_REQUIRE(bn > 0, "tapgemm: no valid N tile (GEGLU needs n % 64 == 0)");
   s.bn = bn;
   s.nb = cdiv(s.n, bn);
@@ -113,6 +118,13 @@ extern "C" {
 int vgen_set_tapgemm_impl(int impl) {
   if (impl < 0 || impl > 1) return fail("vgen_set_tapgemm_impl: impl must be 0 (auto) or 1 (simt)");
   g_tapgemm_impl = impl;
+  return 0;
+}
+
+int vgen_set_tapgemm_bn(int bn) {
+  if (bn != 0 && (bn < 32 || bn > 256 || bn % 32 != 0))
+    return fail("vgen_set_tapgemm_bn: bn must be 0 (heuristic) or a multiple of 32 in [32, 256]");
+  g_tapgemm_bn = bn;
   return 0;
 }
 

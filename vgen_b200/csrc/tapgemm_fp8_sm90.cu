@@ -289,6 +289,7 @@ int vgen_linear_fp8(const void* a, const float* a_scale, int64_t m, int64_t k, i
   if (epi) {
     VG_REQUIRE(!epi->group_bias && !epi->row_stats && !epi->col_sum,
                "vgen_linear_fp8: the e4m3 GEMM takes bias / residual / GEGLU epilogues only");
+    VG_REQUIRE(!(epi->geglu && epi->residual), "vgen_linear_fp8: the GEGLU epilogue takes no residual");
   }
   if (m == 0) return 0;
   const bool geglu = epi && epi->geglu;

@@ -235,6 +235,8 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   VG_REQUIRE((reinterpret_cast<uintptr_t>(a.a) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.w) & 15) == 0,
              "tapgemm_sm90: A and W must be 16-byte aligned");
   if (a.epi.geglu) VG_REQUIRE(s.bn % 64 == 0 && s.n % s.bn == 0, "tapgemm_sm90: GEGLU needs BN%64==0 and N%BN==0");
+  if (a.epi.geglu) VG_REQUIRE(!a.epi.residual && !a.epi.group_bias && (reinterpret_cast<uintptr_t>(a.epi.bias) & 15) == 0,
+                             "tapgemm_sm90: GEGLU takes no residual / per-frame bias and needs a 16-byte aligned bias");
   if (a.epi.row_stats) VG_REQUIRE(!a.epi.residual && !a.epi.group_bias && s.num_taps == 1 && s.d2 == 1 && s.d3 == 1,
                                   "tapgemm: a folded LayerNorm goes with a plain linear (no residual / per-frame bias)");
   if (a.epi.gelu) VG_REQUIRE(s.bn <= kMaxBnGelu, "tapgemm_sm90: the GELU epilogue needs BN <= 224");

@@ -116,6 +116,8 @@ def _epilogue(n_out, bias=None, group_bias=None, residual=None, alpha=1.0, geglu
         e.residual = r2.data_ptr()
         e.residual_ld = ldr
         keep.append(r2)
+    if geglu and residual is not None:
+        raise _l.VgenError("the GEGLU epilogue takes no residual")
     e.geglu = 1 if geglu else 0
     e.bn = int(bn)
     return e, keep
@@ -212,8 +214,9 @@ def linear_fp8(a, w8, w_scale, bias=None, residual=None, alpha=1.0, geglu=False,
     """linear() with e4m3 operands: the fp16 activations `a` are quantised per row (quantize_rows_e4m3), then multiplied
     with the per-channel quantised weight (w8, w_scale from quantize_weight_e4m3) by the FP8 tap-GEMM."""
     lead = a.shape[:-1]
-    a8, a_scale = quantize_rows_e4m3(a)
     n_out = w8.shape[0] // 2 if geglu else w8.shape[0]
+    _epilogue(n_out, bias, None, residual, alpha, geglu, bn)   # refuse a bad epilogue before the quantiser launches
+    a8, a_scale = quantize_rows_e4m3(a)
     if out is None:
         out = torch.empty(*lead, n_out, device=a.device, dtype=torch.float16)
     linear_e4m3(a8, a_scale, w8, w_scale, bias=bias, residual=residual, alpha=alpha, geglu=geglu, out=out, bn=bn)
@@ -321,6 +324,12 @@ def tconv3(x, w, bias=None, residual=None, out=None, bn=0):
 
 def set_tapgemm_impl(impl: str):
     _l.check(_l.load().vgen_set_tapgemm_impl({"auto": 0, "simt": 1}[impl]), "vgen_set_tapgemm_impl")
+
+
+def set_tapgemm_bn(bn: int):
+    """Force the N tile of every fp16 tap-GEMM launch that does not pass its own bn (0 = the heuristic again).  A debug
+    knob: the tests reach each kernel instantiation with it."""
+    _l.check(_l.load().vgen_set_tapgemm_bn(int(bn)), "vgen_set_tapgemm_bn")
 
 
 def pack_geglu_weight(w, bias, bn):
