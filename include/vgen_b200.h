@@ -308,6 +308,24 @@ int vgen_canny(const void* src, int src_u8, int64_t n, int64_t c, int64_t h, int
                int64_t s_y, int64_t s_x, int mode, const double* rand, double low, double high, uint8_t* bytes,
                int32_t* hist, int32_t* thr, uint8_t* cls, int32_t* label, uint8_t* keep, float* out, void* stream);
 
+/* ---- the VideoComposer colour-palette annotator (palette.cu) ---------------------------------------------------- */
+/* Palette.histogram of n frames of 3 channels (RGB), h x w, read at element offset i * s_n + ch * s_c + y * s_y + x * s_x:
+ * src_kind 0 fp32 / 2 fp64 in [0, 1] (widened to fp64), 1 uint8 (linearised through lin, fp64 [256], the sRGB
+ * linearisation of v * (1 / 255)).  Per pixel: Lab in fp64 as skimage 0.22 rgb2lab (D65, 2-degree observer), the nearest
+ * of the npal <= 156 palette entries lab4 (fp64 [npal][4]: L, a, b and |Lab|^2) by -2 x.y + |x|^2 + |y|^2 clipped at 0,
+ * first index on ties; counts into the workspace counts (uint32 [n][npal], zeroed by the call).  Then per frame
+ * count / (h * w), and when weight (fp64 [npal][npal], row-normalised exp(-lab_dists / 2 sigma^2)) is given, the smoothed
+ * histogram weight . hist with values below 1e-5 set to 0.  out: [n][npal], fp64 (out_f64) or fp32.
+ * replaces: tools/annotator/histogram/palette.py:68-81 (rgb2lab, euclidean_distances, argmin, bincount on the host) */
+int vgen_palette_histogram(const void* src, int src_kind, int64_t n, int64_t h, int64_t w, int64_t s_n, int64_t s_c,
+                           int64_t s_y, int64_t s_x, const double* lab4, int64_t npal, const double* lin,
+                           const double* weight, uint32_t* counts, void* out, int out_f64, void* stream);
+/* Palette.quantize_image: the same nearest-entry pass, writing qrgb[k] (fp64 [npal][3], lab2rgb of each entry) of the
+ * chosen entry k to out, fp64 [n][h][w][3].  replaces: tools/annotator/histogram/palette.py:98-103 */
+int vgen_palette_quantize(const void* src, int src_kind, int64_t n, int64_t h, int64_t w, int64_t s_n, int64_t s_c,
+                          int64_t s_y, int64_t s_x, const double* lab4, int64_t npal, const double* lin,
+                          const double* qrgb, double* out, void* stream);
+
 /* DiagonalGaussianDistribution.sample * scale_factor (autoencoder.py:85-90,211-225): moments fp16 [n][p][2*zc]
  * (mean | logvar, channels-last) + fp32 noise [n][zc][p] -> fp32 z [n][zc][p] */
 int vgen_vae_sample(const void* moments, const float* noise, float* z, int64_t n, int64_t zc, int64_t p, float scale,

@@ -3,7 +3,8 @@ DiffusionDDIM.ddim_sample_loop -> UNetSD_T2VBase / UNetSD_I2VGen (and the VideoL
 LoRA / SR600 / HiGen variants, with the VideoComposer condition encoders and the DreamVideo adapters) forward ->
 AutoencoderKL.decode, exposed under the reference's MODEL / DIFFUSION / AUTO_ENCODER registry names (`register()`), and
 the VideoComposer engines' depth annotator (`MiDaS` / `midas_v3`), sketch annotators (`PiDiNet` / `pidinet_bsd`,
-`SketchSimplification` / `sketch_simplification_gan`) and canny annotator (`CannyDetector`, `canny_video`), and DreamVideo's textual-inversion text path
+`SketchSimplification` / `sketch_simplification_gan`), canny annotator (`CannyDetector`, `canny_video`) and colour-palette
+annotator (`Palette`, `histogram_video`), and DreamVideo's textual-inversion text path
 (`FrozenOpenCLIPCustomEmbedder` + `EmbeddingManager`, EMBEDDER / EMBEDMANAGER) with DDIM inversion
 (`DiffusionDDIM.ddim_reverse_sample_loop`), and DreamVideo's evaluation metric (`calculate_metric`, `score_video`,
 `load_clip`, `dino_transform`, with the DINO ViT `vit_small`), and InstructVideo's segmental HPSv2 reward
@@ -49,6 +50,9 @@ def __getattr__(name):  # lazy: importing the package must not require torch.cud
     if name in ("CannyDetector", "canny_video"):
         from . import canny
         return getattr(canny, name)
+    if name in ("Palette", "histogram_video"):
+        from . import palette
+        return getattr(palette, name)
     if name in ("SegmentalReward", "load_hps", "segment_indices"):
         from . import reward
         return getattr(reward, name)

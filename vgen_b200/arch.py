@@ -46,6 +46,7 @@ class UNetPlan:
     context_embedding_depth: int = 0        # higen: depth of TextContextCrossTransformerMultiLayer
     video_compositions: Tuple[str, ...] = ()  # videolcm / tft2v: config.video_compositions (condition encoders built)
     resolution: Tuple[int, ...] = ()        # videolcm / tft2v: config.resolution [W, H]; the stems pool to (H//2, W//2)
+    hist_dim: int = 156                     # videolcm / tft2v with 'histogram': the palette size hist_context_embedding reads
     # DreamVideo adapters (unet_dreamvideo.py:45-51): sites per transformer kind, hidden width (0: width // 2), the temporal
     # adapters' condition width (0: none) and the position ('parallel' | 'serial') of each site
     spatial_adapters: Tuple[str, ...] = ()
@@ -67,7 +68,7 @@ def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, nu
               use_fps_condition=False, concat_dim=8, context_embedding_depth=4, video_compositions=(), resolution=(),
               spatial_adapters=(), temporal_adapters=(), spatial_adapter_hidden=0, temporal_adapter_hidden=0,
               adapter_condition_dim=0, spatial_adapter_positions=(), temporal_adapter_positions=(), lora_rank=0,
-              **_ignored) -> UNetPlan:
+              hist_dim=156, **_ignored) -> UNetPlan:
     """Block layout for the given constructor kwargs (defaults are the reference's own)."""
     if not temporal_attention:
         raise NotImplementedError("temporal_attention=False is not on the sampling hot path")
@@ -85,6 +86,7 @@ def unet_plan(kind, in_dim=4, dim=512, y_dim=512, context_dim=512, out_dim=6, nu
     if kind == "videolcm":
         plan.video_compositions = tuple(video_compositions)
         plan.resolution = tuple(resolution or ())
+        plan.hist_dim = int(hist_dim)
     plan.spatial_adapters, plan.temporal_adapters = tuple(spatial_adapters), tuple(temporal_adapters)
     plan.spatial_adapter_hidden, plan.temporal_adapter_hidden = spatial_adapter_hidden, temporal_adapter_hidden
     plan.adapter_condition_dim = adapter_condition_dim
@@ -262,7 +264,7 @@ VCOMP_NAMES = frozenset(["text", "image", "histogram"] + [c[0] for c in VCOMP_SP
 
 
 def _vcomp_spec(plan: UNetPlan) -> Spec:
-    """pre_image_condition and the condition encoders, unet_videolcm.py:283-372."""
+    """pre_image_condition, the condition encoders and the histogram embedding, unet_videolcm.py:283-380."""
     s: Spec = []
     comps, cd = plan.video_compositions, plan.concat_dim
     if "image" in comps:
@@ -271,6 +273,8 @@ def _vcomp_spec(plan: UNetPlan) -> Spec:
         if name in comps:
             s += _conv(enc + "0.", cd * 4, cin, 3, 3) + _conv(enc + "3.", cd * 4, cd * 4, 3, 3) + _conv(enc + "5.", cd, cd * 4, 3, 3)
             s += _transformer_v2(after, cd)
+    if "histogram" in comps:   # Linear(hist_dim, embed_dim) -> SiLU -> Linear(embed_dim, context_dim), :374-380
+        s += _mlp("hist_context_embedding.", plan.hist_dim, plan.embed_dim, plan.context_dim)
     return s
 
 

@@ -103,6 +103,9 @@ _SIGNATURES = {
     "vgen_segment_reward": [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _f32, _vp, _vp],
     "vgen_canny": [_vp, _i32, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _vp, _f64, _f64, _vp, _vp, _vp, _vp,
                    _vp, _vp, _vp, _vp],
+    "vgen_palette_histogram": [_vp, _i32, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i32,
+                               _vp],
+    "vgen_palette_quantize": [_vp, _i32, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _vp],
 }
 _RESTYPES = {"vgen_last_error": ctypes.c_char_p, "vgen_launch_count": ctypes.c_int64,
              "vgen_group_norm_workspace_bytes": ctypes.c_int64}

@@ -632,6 +632,16 @@ def copy2d(src, dst):
     return dst
 
 
+def broadcast_row(src, dst):
+    """dst[r, :] = src for every row r of the 2-D row view dst (src: a contiguous 1-D tensor of dst's width)."""
+    d2, ldd = _rows_view(dst, "dst")
+    if src.dim() != 1 or not src.is_contiguous() or src.shape[0] != d2.shape[1] or src.dtype != d2.dtype:
+        raise _l.VgenError("broadcast_row: src must be a contiguous row of dst's width and dtype")
+    rc = _l.load().vgen_copy2d(_p(src), 0, _p(d2), ldd, d2.shape[0], d2.shape[1], _stream())
+    _l.check(rc, "vgen_copy2d")
+    return dst
+
+
 def concat_channels(a, b):
     """torch.cat([a, b], dim=-1) for channels-last tensors with equal leading dims."""
     ca, cb = a.shape[-1], b.shape[-1]
@@ -1190,3 +1200,66 @@ def canny(frames, mode, rand=None, low=0.0, high=0.0, out=None, thresholds=False
                                            _stream()))
     _l.check(rc, "vgen_canny")
     return (out, thr) if thresholds else out
+
+
+# ------------------------------------------------------------------------------------------------
+# the VideoComposer colour-palette annotator (palette.cu)
+_PAL_KIND = {torch.float32: 0, torch.uint8: 1, torch.float64: 2}
+
+
+def _palette_src(frames, name, lab4, lin):
+    if not frames.is_cuda or frames.dtype not in _PAL_KIND:
+        raise _l.VgenError(f"{name}: frames must be a CUDA fp32, fp64 or uint8 tensor, got {frames.dtype} on {frames.device}")
+    if frames.dim() != 4 or frames.shape[1] != 3 or frames.shape[2] == 0 or frames.shape[3] == 0:
+        raise _l.VgenError(f"{name}: frames must be [n, 3, h, w] (any strides), got {tuple(frames.shape)}")
+    dev = frames.device
+    npal = lab4.shape[0] if lab4.dim() == 2 else -1
+    if lab4.dtype != torch.float64 or lab4.device != dev or not lab4.is_contiguous() or lab4.shape[-1] != 4 \
+            or not 1 <= npal <= 156:
+        raise _l.VgenError(f"{name}: the palette table must be a contiguous fp64 [npal, 4] tensor on {dev} with 1 to 156 "
+                           f"entries (the UNet's hist_dim), got {tuple(lab4.shape)}")
+    if frames.dtype == torch.uint8 and (lin is None or lin.dtype != torch.float64 or lin.device != dev
+                                        or tuple(lin.shape) != (256,) or not lin.is_contiguous()):
+        raise _l.VgenError(f"{name}: uint8 frames need the contiguous fp64 [256] linearisation table on {dev}")
+    return _PAL_KIND[frames.dtype], npal
+
+
+def palette_histogram(frames, lab4, lin=None, weight=None, out_dtype=torch.float32):
+    """Palette.histogram of frames [n, 3, h, w] (any element strides; CUDA fp32 / fp64 in [0, 1], or uint8) against the
+    palette lab4 (fp64 [npal, 4]: L, a, b, |Lab|^2; npal <= 156) -> [n, npal] of out_dtype (fp32 or fp64).  lin: the
+    uint8 linearisation table (fp64 [256]); weight: the row-normalised smoothing matrix (fp64 [npal, npal]) or None
+    (sigma <= 0: the plain normalised counts, no zeroing)."""
+    kind, npal = _palette_src(frames, "palette_histogram", lab4, lin)
+    dev = frames.device
+    if weight is not None and (weight.dtype != torch.float64 or weight.device != dev or not weight.is_contiguous()
+                               or tuple(weight.shape) != (npal, npal)):
+        raise _l.VgenError(f"palette_histogram: weight must be a contiguous fp64 [{npal}, {npal}] tensor on {dev}")
+    if out_dtype not in (torch.float32, torch.float64):
+        raise _l.VgenError(f"palette_histogram: out_dtype must be fp32 or fp64, got {out_dtype}")
+    n, _, h, w = frames.shape
+    counts = torch.empty(n, npal, device=dev, dtype=torch.int32)
+    out = torch.empty(n, npal, device=dev, dtype=out_dtype)
+    s_n, s_c, s_y, s_x = frames.stride()
+    rc = _run("palette", 1250.0 * n * h * w, n * h * w * 3 * frames.element_size(),
+              lambda: _l.load().vgen_palette_histogram(_p(frames), kind, n, h, w, s_n, s_c, s_y, s_x, _p(lab4), npal,
+                                                       _p(lin) if kind == 1 else None, _p(weight), _p(counts), _p(out),
+                                                       1 if out_dtype == torch.float64 else 0, _stream()))
+    _l.check(rc, "vgen_palette_histogram")
+    return out
+
+
+def palette_quantize(frames, lab4, qrgb, lin=None):
+    """Palette.quantize_image of frames [n, 3, h, w] (as palette_histogram) -> fp64 [n, h, w, 3]: qrgb[k] (fp64 [npal, 3],
+    lab2rgb of each palette entry) of each pixel's nearest entry k."""
+    kind, npal = _palette_src(frames, "palette_quantize", lab4, lin)
+    dev = frames.device
+    if qrgb.dtype != torch.float64 or qrgb.device != dev or not qrgb.is_contiguous() or tuple(qrgb.shape) != (npal, 3):
+        raise _l.VgenError(f"palette_quantize: qrgb must be a contiguous fp64 [{npal}, 3] tensor on {dev}")
+    n, _, h, w = frames.shape
+    out = torch.empty(n, h, w, 3, device=dev, dtype=torch.float64)
+    s_n, s_c, s_y, s_x = frames.stride()
+    rc = _run("palette", 1250.0 * n * h * w, n * h * w * (3 * frames.element_size() + 24),
+              lambda: _l.load().vgen_palette_quantize(_p(frames), kind, n, h, w, s_n, s_c, s_y, s_x, _p(lab4), npal,
+                                                      _p(lin) if kind == 1 else None, _p(qrgb), _p(out), _stream()))
+    _l.check(rc, "vgen_palette_quantize")
+    return out

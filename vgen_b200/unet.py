@@ -306,6 +306,8 @@ class _UNetBase(SpecModule):
             comps = self.plan.video_compositions
             if "image" in comps:
                 lin("pre_image_condition.0."), lin("pre_image_condition.2.")
+            if "histogram" in comps:
+                lin("hist_context_embedding.0."), lin("hist_context_embedding.2.")
             for name, _kw, enc, after, _cin in arch.VCOMP_SPATIAL:
                 if name in comps:
                     # the stem conv stays fp32 [cout][cin][3][3] (ops.cond_stem); the stride-2 convs are tap-GEMM packed
@@ -422,16 +424,36 @@ class _UNetBase(SpecModule):
         return ops.linear_gelu_rowbias(t, ad["down.w"], bias=ad["down.b"], row_bias=g,
                                        rows_per_group=(cond[1] * hw if g is not None else 1), out=out)
 
+    @staticmethod
+    def _frame_kv(shared, own, w, f):
+        """Cross-attention K/V of a per-frame context [y tokens | image tokens | the frame's own token]: the shared tokens
+        shared [b, L, ctx_dim] go through the K/V GEMM once per video, the per-frame tokens own [(b f), ctx_dim] once per
+        frame; both are copied into kv [(b f), L + 1, 2 inner]."""
+        b, lctx, cdim = shared.shape
+        kv_s = ops.linear(shared.view(-1, cdim), w)                      # [b L, 2 inner]
+        kv_o = ops.linear(own, w)                                       # [(b f), 2 inner]
+        width = w.shape[0]
+        kv = torch.empty(b * f, lctx + 1, width, device=own.device, dtype=torch.float16)
+        rows = kv.view(b, f, (lctx + 1) * width)
+        for i in range(b):
+            ops.broadcast_row(kv_s[i * lctx:(i + 1) * lctx].reshape(-1), rows[i, :, :lctx * width])
+        ops.copy2d(kv_o, kv.view(b * f, (lctx + 1) * width)[:, lctx * width:])
+        return kv
+
     def _basic_block_spatial(self, t, ctx_tokens, W, p, heads, n, hw, inner, f):
-        """BasicTransformerBlock on tokens t [M, inner] (M = n*hw); ctx_tokens [b, L, ctx_dim] fp16."""
+        """BasicTransformerBlock on tokens t [M, inner] (M = n*hw); ctx_tokens [b, L, ctx_dim] fp16 shared by the f frames
+        of a video, or (shared [b, L, ctx_dim], per-frame tokens [(b f), ctx_dim]) when each frame appends its own token."""
         t = self._sublayer_out(t, W, p, "attn_adapter", "attn1.to_out.0.", inner, hw, lambda o: ops.attention_d64(
             *self._self_attn_qkv_spatial(t, W, p + "attn1.", p + "norm1.", n, hw, inner), heads,
             out=None if o is None else o.view(n, hw, inner)))
         q = self._ln_linear(t, W, p + "attn2.q", p + "norm2.").view(n, hw, inner)
-        bctx, lctx, cdim = ctx_tokens.shape
-        kv = ops.linear(ctx_tokens.view(-1, cdim), W[p + "attn2.kv"]).view(bctx, lctx, 2 * inner)
+        if isinstance(ctx_tokens, tuple):
+            kv, div = self._frame_kv(*ctx_tokens, W[p + "attn2.kv"], f), 1
+        else:
+            bctx, lctx, cdim = ctx_tokens.shape
+            kv, div = ops.linear(ctx_tokens.view(-1, cdim), W[p + "attn2.kv"]).view(bctx, lctx, 2 * inner), f
         t = self._sublayer_out(t, W, p, "cross_attn_adapter", "attn2.to_out.0.", inner, hw, lambda o: ops.attention_d64(
-            q, kv[:, :, :inner], kv[:, :, inner:], heads, kv_batch_div=f, out=None if o is None else o.view(n, hw, inner)))
+            q, kv[:, :, :inner], kv[:, :, inner:], heads, kv_batch_div=div, out=None if o is None else o.view(n, hw, inner)))
         return self._feed_forward(t, W, p, hw)
 
     def _feed_forward(self, t, W, p, hw=1):
@@ -684,17 +706,24 @@ class UNetSD_VideoLCM(_UNetBase):
     config.resolution / 2 in one kernel), two stride-2 convs and a Transformer_v2 over the frames; the encodings are summed
     in the reference's order into the concat_dim channels next to x (:598-703).  'image' adds num_tokens context tokens
     after the text tokens (pre_image_condition, :743-745).  A listed condition passed as None contributes nothing, as in
-    the reference.  'histogram' (per-frame context tokens, no released config) and config.use_text_clip_vip_model raise."""
+    the reference.  'histogram' (hist_context_embedding, :374-380,751-759) turns a histogram [b, f, hist_dim]
+    (vgen_b200.palette.histogram_video) into one more context token per frame, after the shared text and image tokens;
+    the cross attention then reads a per-frame context.  No released config or checkpoint has it, so it is opt-in: a
+    config listing 'histogram' builds only with the constructor keyword enable_histogram=True (a YAML UNet: dict can set
+    it, like fp8_linear) and raises NotImplementedError otherwise, as does a histogram passed to a model built without
+    it.  config.use_text_clip_vip_model raises."""
     KIND = "videolcm"
 
-    def __init__(self, config=None, *args, **kwargs):
+    def __init__(self, config=None, *args, enable_histogram=False, **kwargs):
         comps = list(_cfg_get(config, "video_compositions", None) or ["text"])
         unknown = sorted(set(comps) - arch.VCOMP_NAMES)
         if unknown:
             raise ValueError(f"vgen_b200 {type(self).__name__}: unknown video_compositions {unknown}")
-        if "histogram" in comps:
+        if not isinstance(enable_histogram, bool):
+            raise ValueError(f"vgen_b200: enable_histogram must be True or False, got {enable_histogram!r}")
+        if "histogram" in comps and not enable_histogram:
             raise NotImplementedError(f"vgen_b200 {type(self).__name__}: the 'histogram' composition (per-frame context "
-                                      "tokens) is not supported")
+                                      "tokens) is built only on request: pass enable_histogram=True")
         if _cfg_get(config, "use_text_clip_vip_model", False):
             raise NotImplementedError(f"vgen_b200 {type(self).__name__}: config.use_text_clip_vip_model is not supported")
         if "mask" in comps and not kwargs.get("inpainting", True):
@@ -704,13 +733,14 @@ class UNetSD_VideoLCM(_UNetBase):
         if self._spatial and (res is None or len(res) != 2):
             raise ValueError(f"vgen_b200 {type(self).__name__}: spatial compositions need config.resolution = [W, H]")
         self._comps, self._res = comps, tuple(res) if res is not None else ()
+        self._hist_dim = int(kwargs.get("hist_dim", 156))
         super().__init__(config, *args, **kwargs)
         self.video_compositions = comps
         self.resolution = self._res
         self.concat_dim = self.plan.concat_dim
 
     def _plan_kwargs(self, config):
-        return dict(video_compositions=tuple(self._comps), resolution=self._res)
+        return dict(video_compositions=tuple(self._comps), resolution=self._res, hist_dim=self._hist_dim)
 
     def _encode_condition(self, v, kw, W, b, f, h, w):
         """<kw>_embedding + <kw>_embedding_after (unet_videolcm.py:599-699) -> tokens [(b f h w), concat_dim] fp16."""
@@ -735,8 +765,6 @@ class UNetSD_VideoLCM(_UNetBase):
                 focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0, **kwargs):
         self._check_x(x, t)
         name = type(self).__name__
-        if histogram is not None:
-            raise NotImplementedError(f"vgen_b200 {name}: the 'histogram' condition is not supported")
         conds = dict(depth=depth, local_image=local_image, motion=motion, canny=canny, sketch=sketch,
                      single_sketch=single_sketch, masked=masked)
         for kw, v in conds.items():
@@ -745,8 +773,15 @@ class UNetSD_VideoLCM(_UNetBase):
                                  f"video_compositions {self.video_compositions}")
         if image is not None and "image" not in self.video_compositions:
             raise ValueError(f"vgen_b200 {name}: 'image' was passed but is not in video_compositions {self.video_compositions}")
-        W = self._packed or self._pack()
         b, c, f, h, w = x.shape
+        if histogram is not None:
+            if "histogram" not in self.video_compositions:
+                raise NotImplementedError(f"vgen_b200 {name}: the 'histogram' condition needs a model built with "
+                                          "'histogram' in video_compositions and enable_histogram=True")
+            if tuple(histogram.shape) != (b, f, self.plan.hist_dim) or not histogram.is_cuda:
+                raise ValueError(f"vgen_b200 {name}: histogram must be a CUDA tensor [{b}, {f}, {self.plan.hist_dim}], "
+                                 f"got {tuple(histogram.shape)} on {histogram.device}")
+        W = self._packed or self._pack()
         concat = None
         for kw in arch.VCOMP_SUM_ORDER:
             if conds[kw] is not None:
@@ -762,6 +797,9 @@ class UNetSD_VideoLCM(_UNetBase):
             img = self._to_f16_rows(image.reshape(b, -1, image.shape[-1]))
             parts.append(self._mlp(img.view(-1, img.shape[-1]), W, "pre_image_condition.").view(b, self.num_tokens, self.context_dim))
         ctx = self._context(parts, b)
+        if histogram is not None:                                   # one token per frame after the shared ones (:751-759)
+            hist = self._to_f16_rows(histogram)
+            ctx = (ctx, self._mlp(hist.view(b * f, -1), W, "hist_context_embedding."))
         cin = self.plan.input_blocks[0][0].cin                      # in_dim + concat_dim; the concat channels are 0 without conditions
         cpad = ((cin + 7) // 8) * 8
         xin = ops.cp_to_pc(x.contiguous(), b, c, f * h * w, c_pad=cpad).view(b * f, h, w, cpad)
