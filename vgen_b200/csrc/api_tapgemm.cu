@@ -14,7 +14,12 @@ static int g_tapgemm_bn = 0;    // 0 = pick_bn; else the N tile of every launch 
 // epilogue / pipeline fill).  With FEW M tiles (the coarse levels of the UNet) the persistent grid runs
 // ceil(tiles / SMs) waves and the widest tile can leave most of the last wave idle, while a narrower one adds a wave
 // of less work each.  So the cost is waves x (BN + overhead), waves counted on this device.
-static int pick_bn(long n, int geglu, long m_tiles, int ctas, int max_bn) {
+// The widest candidate is 224: on every tap-GEMM shape of bench.py's i2vgen step, BN = 256 measured no faster than the
+// best narrower tile except on two 22 x 40 conv3x3s with K >= 17 280 (within 2 % there), and 1.2-1.5x slower on the
+// 1280-wide linears and temporal convs (K = 1280 ... 5120), which the model used to give 256 (H100 80GB HBM3, 700 W;
+// tools/bench_tapgemm_wide.py).  GEGLU keeps its own rule: its tile is fixed when the weight is packed.
+static constexpr int kMaxBnAuto = 224;
+static int pick_bn(long n, int geglu, long m_tiles, int ctas) {
   if (geglu) {
     for (int bn = 256; bn >= 64; bn -= 64)
       if (n % bn == 0) return bn;
@@ -24,7 +29,7 @@ static int pick_bn(long n, int geglu, long m_tiles, int ctas, int max_bn) {
   if (ctas < 1) ctas = 1;
   int best = 128;
   double best_cost = 1e30;
-  for (int bn = max_bn; bn >= 96; bn -= 32) {
+  for (int bn = kMaxBnAuto; bn >= 96; bn -= 32) {
     const long nb = (n + bn - 1) / bn;
     const long tiles = nb * (m_tiles > 0 ? m_tiles : 1);
     const long waves = (tiles + ctas - 1) / ctas;
@@ -94,7 +99,7 @@ static int finish_and_launch(TapGemmArgs* t, const vgen_epilogue* epi, void* str
   const long m_tiles_all = (long)s.d3 * cdiv(s.d2, s.box2) * cdiv(s.d1, s.box1);
   int bn = (epi && epi->bn > 0) ? epi->bn
            : g_tapgemm_bn > 0   ? g_tapgemm_bn
-                                : pick_bn(s.n, t->epi.geglu, m_tiles_all, sm_count(), t->epi.gelu ? kMaxBnGelu : 256);
+                                : pick_bn(s.n, t->epi.geglu, m_tiles_all, sm_count());
   VG_REQUIRE(bn > 0, "tapgemm: no valid N tile (GEGLU needs n % 64 == 0)");
   s.bn = bn;
   s.nb = cdiv(s.n, bn);

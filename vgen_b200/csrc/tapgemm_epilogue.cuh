@@ -124,6 +124,7 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
       }
   }
   __half* orow[2] = {e.out + t.ooff[0], e.out + t.ooff[1]};
+  constexpr bool kResidual = !kLn && !kGelu && !kRelu;   // the launchers refuse a residual with the other epilogues
   if constexpr (!kGeglu) {
     const int n0 = t.nb_i * BN;
     const __half* grow = e.group_bias ? e.group_bias + (long)fd_div(e.f_group_bias_div, t.i3) * e.ld_group_bias : nullptr;
@@ -140,6 +141,28 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
       const bool full = nbase + 32 <= s.n;
       const bool vec = vec_ok && full;               // pairs are loaded / stored as 4- or 8-byte words
       const bool staged = st.tma && vec;             // uniform over the CTA
+      // The chunk's residual pairs are loaded up front, all in flight together: the staging stores below carry a
+      // "memory" clobber, so a load left in the loop would wait for the previous store and the chunk would pay one
+      // DRAM latency per pair.
+      __half2 res[4][2];
+      if (kResidual && e.residual) {
+#pragma unroll
+        for (int g4 = 0; g4 < 4; ++g4) {
+          const int n = nbase + g4 * 8 + q2;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            res[g4][h] = __float2half2_rn(0.f);
+            if (!t.row_ok[h]) continue;
+            const __half* rrow = e.residual + t.row[h] * e.ldr;
+            if (vec) {
+              res[g4][h] = __ldg(reinterpret_cast<const __half2*>(rrow + n));
+            } else {
+              if (n < s.n) res[g4][h].x = rrow[n];
+              if (n + 1 < s.n) res[g4][h].y = rrow[n + 1];
+            }
+          }
+        }
+      }
       if (staged) epi_stage_acquire(st);
 #pragma unroll
       for (int g4 = 0; g4 < 4; ++g4) {
@@ -193,16 +216,9 @@ __device__ __forceinline__ void tapgemm_epilogue_tile(const TapGemmShape& s, con
             f0 = round_h(f0) + gb.x;
             f1 = round_h(f1) + gb.y;
           }
-          if (!kLn && e.residual && t.row_ok[h]) {
-            const __half* rrow = e.residual + t.row[h] * e.ldr;
-            if (vec) {
-              const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(rrow + n)));
-              f0 = round_h(f0) + r.x;
-              f1 = round_h(f1) + r.y;
-            } else {
-              if (n < s.n) f0 = round_h(f0) + __half2float(rrow[n]);
-              if (n + 1 < s.n) f1 = round_h(f1) + __half2float(rrow[n + 1]);
-            }
+          if (kResidual && e.residual && t.row_ok[h]) {
+            if (vec || n < s.n) f0 = round_h(f0) + __low2float(res[g4][h]);
+            if (vec || n + 1 < s.n) f1 = round_h(f1) + __high2float(res[g4][h]);
           }
           if (staged) {
             epi_stage_put(st, h, g4, pack_half2(f0, f1));   // rows outside the tensor are clipped by the TMA unit

@@ -215,7 +215,7 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
     if (kind == 3) launch_kernel(tapgemm_sm90_kernel<BN, 3>, dim3(grid), dim3(kThreads), smem, stream, p);
     if (kind == 1) launch_kernel(tapgemm_sm90_kernel<BN, 1>, dim3(grid), dim3(kThreads), smem, stream, p);
   }
-  if constexpr (BN < 256) {   // the GELU epilogue spills at BN = 256: the launcher never picks it (kMaxBnGelu)
+  if constexpr (BN < 256) {   // the GELU epilogue spills at BN = 256: pick_bn stops at 224, a forced 256 is refused
     if (kind == 4) launch_kernel(tapgemm_sm90_kernel<BN, 4>, dim3(grid), dim3(kThreads), smem, stream, p);
   }
   if (kind == 8) launch_kernel(tapgemm_sm90_kernel<BN, 8>, dim3(grid), dim3(kThreads), smem, stream, p);
