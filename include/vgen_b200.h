@@ -67,6 +67,27 @@ typedef struct vgen_epilogue {
 int vgen_linear(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, void* out,
                 int64_t ldo, const vgen_epilogue* epi, void* stream);
 
+/* vgen_linear with a K tail (UNetSD_LoRA's runtime LoRA):
+ *   out[m][n] = epi(a[m][:k] . w[n][:k] + h[m][:r] . u[n][:r])
+ * both products accumulate into the same fp32 accumulator before the epilogue (bias, residual, one fp16 rounding).  h fp16
+ * [m][r] (row stride ldh) is the strength-scaled LoRA down projection of a (vgen_lora_down), u fp16 [n][r] the up weights
+ * of every set side by side (block-diagonal over the q / k / v row blocks of a fused projection); r a multiple of 64
+ * (zero-padded), h / u 16-byte aligned, ldh a multiple of 8.  epi: alpha, bias, residual, bn; no group_bias, GEGLU or
+ * folded LayerNorm.  Same kernels as vgen_linear (vgen_set_tapgemm_impl, vgen_set_tapgemm_bn).
+ * replaces: to_q(x) + to_q_lora(x) * scale and the same for k, v and out, tools/modules/unet/unet_lora.py:114-131,161-195 */
+int vgen_linear_lora(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, const void* h, int64_t r,
+                     int64_t ldh, const void* u, void* out, int64_t ldo, const vgen_epilogue* epi, void* stream);
+/* LoRA down projection with the per-sample strength folded in (lora.cu):
+ *   h[row][j] = fp16(strength[row / rows_per_sample][col_set[j]] * col_scale[j] * (x[row][:k] . d[j][:k]))   j < r
+ *   h[row][j] = 0                                                                                            r <= j < r_pad
+ * x fp16 [m][k] (row stride ldx), d fp16 [r][k] (the down weights of every set and every projection reading x, stacked),
+ * col_set int32 [r] (the set of column j, < nsets), col_scale fp32 [r] (alpha / rank of that set), strength fp32
+ * [m / rows_per_sample][nsets], h fp16 [m][ldh].  k a multiple of 8 up to 2560, x / d 16-byte aligned.
+ * replaces: to_q_lora.down_linear(x) (and k, v, out), unet_lora.py:114-131 */
+int vgen_lora_down(const void* x, int64_t m, int64_t k, int64_t ldx, const void* d, int64_t r, const int32_t* col_set,
+                   const float* col_scale, const float* strength, int64_t nsets, int64_t rows_per_sample, void* h,
+                   int64_t ldh, int64_t r_pad, void* stream);
+
 /* Adapter down projection (DreamVideo, tools/modules/unet/util.py:499-519):
  *   out[m][j] = fp16(gelu_erf(a[m][:k] . w[j][:k] + bias[j] + row_bias[m / rows_per_group][j]))
  * with the fp32 row bias added to the fp32 accumulator before the activation (it carries the adapter's condition term

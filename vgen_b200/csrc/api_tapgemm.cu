@@ -162,6 +162,40 @@ int vgen_linear(const void* a, int64_t m, int64_t k, int64_t lda, const void* w,
   return finish_and_launch(&t, epi, stream);
 }
 
+int vgen_linear_lora(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, const void* h, int64_t r,
+                     int64_t ldh, const void* u, void* out, int64_t ldo, const vgen_epilogue* epi, void* stream) {
+  VG_REQUIRE(a && w && out && h && u, "vgen_linear_lora: null pointer");
+  VG_REQUIRE(m >= 0 && k > 0 && n > 0 && lda >= k && r > 0 && r % 64 == 0 && ldh >= r, "vgen_linear_lora: bad shape");
+  if (m == 0) return 0;
+  TapGemmArgs t{};
+  t.a = reinterpret_cast<const __half*>(a);
+  t.w = reinterpret_cast<const __half*>(w);
+  t.a_stride1 = lda;
+  t.a_stride2 = lda * m;
+  t.a_stride3 = lda * m;
+  t.h = reinterpret_cast<const __half*>(h);
+  t.ldh = ldh;
+  t.u = reinterpret_cast<const __half*>(u);
+  t.r = (int)r;
+  TapGemmShape& s = t.shape;
+  s.c = (int)k;
+  s.d1 = (int)m;
+  s.d2 = 1;
+  s.d3 = 1;
+  s.box1 = 128;
+  s.box2 = 1;
+  s.num_taps = 1;
+  s.tap1[0] = s.tap2[0] = s.tap3[0] = 0;
+  s.n = (int)n;
+  {
+    int rc = fill_epilogue(&t, out, ldo, epi);
+    if (rc) return rc;
+  }
+  VG_REQUIRE(!t.epi.group_bias && !t.epi.geglu && !t.epi.row_stats,
+             "vgen_linear_lora: bias and residual only (no group_bias, GEGLU or folded LayerNorm)");
+  return finish_and_launch(&t, epi, stream);
+}
+
 int vgen_linear_gelu_rowbias(const void* a, int64_t m, int64_t k, int64_t lda, const void* w, int64_t n, const float* bias,
                              const float* row_bias, int64_t ld_row_bias, int64_t rows_per_group, void* out, int64_t ldo,
                              void* stream) {

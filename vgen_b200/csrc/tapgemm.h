@@ -89,6 +89,12 @@ struct TapGemmArgs {
   const __half* a;
   long a_stride1, a_stride2, a_stride3;  // element strides of d1, d2, d3 (channel stride is 1)
   const __half* w;                       // [n][num_taps * c], K-major
+  // K tail (linear only, vgen_linear_lora): out += h[row][:r] . u[n][:r] accumulated after the main K loop into the same
+  // fp32 accumulators; r = 0: none.  h fp16 [rows][r] (row stride ldh), u fp16 [n][r]; r a multiple of 64.
+  const __half* h;
+  long ldh;
+  const __half* u;
+  int r;
   TapGemmShape shape;
   TapGemmEpilogue epi;
 };

@@ -11,7 +11,8 @@ namespace vg {
 __device__ __forceinline__ float gelu_erf_s(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
 __global__ void tapgemm_simt_kernel(const __half* __restrict__ A, long st1, long st2, long st3,
-                                    const __half* __restrict__ W, TapGemmShape s, TapGemmEpilogue e) {
+                                    const __half* __restrict__ W, const __half* __restrict__ H, long ldh,
+                                    const __half* __restrict__ U, int r, TapGemmShape s, TapGemmEpilogue e) {
   const long rows = (long)s.d1 * s.d2 * s.d3;
   const int out_n = e.geglu ? s.n / 2 : s.n;
   const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -32,6 +33,8 @@ __global__ void tapgemm_simt_kernel(const __half* __restrict__ A, long st1, long
       const __half* wp = W + (long)wrow * ktot + (long)t * s.c;
       for (int c = 0; c < s.c; ++c) acc += __half2float(ap[c]) * __half2float(wp[c]);
     }
+    // K tail (linear only): the same accumulator continues over h[row] . u[wrow]
+    for (int j = 0; j < r; ++j) acc += __half2float(H[row * ldh + j]) * __half2float(U[(long)wrow * r + j]);
     return acc;
   };
 
@@ -77,8 +80,10 @@ int tapgemm_simt_launch(const TapGemmArgs& a, cudaStream_t stream) {
   const int threads = 256;
   const long blocks = (total + threads - 1) / threads;
   VG_REQUIRE(blocks < (1L << 31), "tapgemm_simt: problem too large");
-  launch_kernel(tapgemm_simt_kernel, dim3((unsigned)blocks), dim3(threads), 0, stream, a.a, a.a_stride1, a.a_stride2, a.a_stride3, a.w, s,
-                                                               a.epi);
+  VG_REQUIRE(!a.r || (s.num_taps == 1 && s.d2 == 1 && s.d3 == 1 && !a.epi.geglu),
+             "tapgemm_simt: the K tail goes with a plain linear");
+  launch_kernel(tapgemm_simt_kernel, dim3((unsigned)blocks), dim3(threads), 0, stream, a.a, a.a_stride1, a.a_stride2, a.a_stride3, a.w,
+                a.h, a.ldh, a.u, a.r, s, a.epi);
   VG_LAUNCH_CHECK("tapgemm_simt_kernel");
   return 0;
 }

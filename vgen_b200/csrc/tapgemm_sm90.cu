@@ -44,16 +44,21 @@ struct alignas(64) TapGemmKernelParams {
   TapGemmShape s;
   TapGemmEpilogue e;
   int stages;
+  CUtensorMap map_h;    // K tail (kEpi bit 4): H [rows][r] as a rank-4 map shaped like map_a, and U [n][r]
+  CUtensorMap map_u;
+  int tail_iters;       // r / 64
 };
 
 // kEpi: bit 0 = GEGLU epilogue, bit 1 = LayerNorm folded into the epilogue (TapGemmEpilogue.row_stats), bit 2 = GELU with the
-// fp32 row bias (TapGemmEpilogue.gelu), bit 3 = ReLU (TapGemmEpilogue.relu); BN (the wgmma N and the accumulator count) is a
+// fp32 row bias (TapGemmEpilogue.gelu), bit 3 = ReLU (TapGemmEpilogue.relu), bit 4 = K tail (TapGemmArgs.h / u: r / 64 more
+// k-iterations after the main loop, H and U tiles loaded through their own maps into the same ring stages); BN (the wgmma N and the accumulator count) is a
 // template parameter as well, so every register index of the epilogue is a constant.
 template <int BN, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_constant__ TapGemmKernelParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atom (8 rows x 128 B).
   constexpr bool kGeglu = (kEpi & 1) != 0, kLn = (kEpi & 2) != 0, kGelu = (kEpi & 4) != 0, kRelu = (kEpi & 8) != 0;
+  constexpr bool kTail = (kEpi & 16) != 0;
   constexpr int kBBytes = BN * kBK * 2;                            // multiple of 1024 (BN % 32 == 0)
   constexpr int kStageBytes = kABytes + kBBytes;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -69,13 +74,17 @@ __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_
   uint64_t* empty_bar = full_bar + stages;                                          // [stages]
 
   const TapGemmShape& s = p.s;
-  const int k_iters = s.num_taps * s.kc;
+  const int k_iters = s.num_taps * s.kc + (kTail ? p.tail_iters : 0);
   const uint32_t stage_tx = (uint32_t)(s.box1 * s.box2 * kBK * 2 + kBBytes);
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.map_a);
     tma_prefetch_desc(&p.map_b);
     if (p.out_tma) tma_prefetch_desc(&p.map_out);
+    if constexpr (kTail) {
+      tma_prefetch_desc(&p.map_h);
+      tma_prefetch_desc(&p.map_u);
+    }
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
@@ -107,6 +116,22 @@ __global__ void __launch_bounds__(kThreads, 1) tapgemm_sm90_kernel(const __grid_
             uint8_t* sa = tiles + (size_t)st * kStageBytes;
             tma_load_4d(sa, &p.map_a, &full_bar[st], kc_i * kBK, c1, c2, c3);
             tma_load_2d(sa + kABytes, &p.map_b, &full_bar[st], wk0 + kc_i * kBK, n0);
+          }
+          __syncwarp();
+          if (++st == stages) {
+            st = 0;
+            ph ^= 1;
+          }
+        }
+      }
+      if constexpr (kTail) {   // the tail tiles have the main loop's A / B tile shapes, so the consumers cannot tell them apart
+        for (int r = 0; r < p.tail_iters; ++r) {
+          mbar_wait(&empty_bar[st], ph ^ 1);
+          if (elect_one()) {
+            mbar_expect_tx(&full_bar[st], stage_tx);
+            uint8_t* sa = tiles + (size_t)st * kStageBytes;
+            tma_load_4d(sa, &p.map_h, &full_bar[st], r * kBK, i1_0, i2_0, i3);
+            tma_load_2d(sa + kABytes, &p.map_u, &full_bar[st], r * kBK, n0);
           }
           __syncwarp();
           if (++st == stages) {
@@ -203,6 +228,7 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if constexpr (BN < 256)
       VG_CUDA(cudaFuncSetAttribute(tapgemm_sm90_kernel<BN, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if constexpr (BN % 64 == 0) {
@@ -218,6 +244,7 @@ static int launch_bn(const TapGemmKernelParams& p, int kind, int grid, size_t sm
   if constexpr (BN < 256) {   // the GELU epilogue spills at BN = 256: pick_bn stops at 224, a forced 256 is refused
     if (kind == 4) launch_kernel(tapgemm_sm90_kernel<BN, 4>, dim3(grid), dim3(kThreads), smem, stream, p);
   }
+  if (kind == 16) launch_kernel(tapgemm_sm90_kernel<BN, 16>, dim3(grid), dim3(kThreads), smem, stream, p);
   if (kind == 8) launch_kernel(tapgemm_sm90_kernel<BN, 8>, dim3(grid), dim3(kThreads), smem, stream, p);
   if (kind == 2) launch_kernel(tapgemm_sm90_kernel<BN, 2>, dim3(grid), dim3(kThreads), smem, stream, p);
   if (kind == 0) launch_kernel(tapgemm_sm90_kernel<BN, 0>, dim3(grid), dim3(kThreads), smem, stream, p);
@@ -245,6 +272,9 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   if (a.epi.relu) VG_REQUIRE(!a.epi.geglu && !a.epi.row_stats && !a.epi.gelu && !a.epi.residual && !a.epi.group_bias,
                              "tapgemm: the ReLU epilogue goes with bias only");
   VG_REQUIRE(!a.epi.out_s2 || a.epi.relu, "tapgemm_sm90: a strided output goes with the ReLU epilogue");
+  if (a.r) VG_REQUIRE(a.r % 64 == 0 && s.num_taps == 1 && s.d2 == 1 && s.d3 == 1 && !a.epi.geglu && !a.epi.row_stats &&
+                      !a.epi.gelu && !a.epi.relu && !a.epi.group_bias,
+                      "tapgemm_sm90: the K tail goes with a plain linear (bias / residual only), r a multiple of 64");
 
   TapGemmKernelParams p;
   p.s = s;
@@ -264,6 +294,21 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
     const uint64_t strides[1] = {(uint64_t)s.num_taps * s.c * 2};
     const uint32_t box[2] = {64, (uint32_t)s.bn};
     int rc = make_tmap_f16(&p.map_b, a.w, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  p.tail_iters = a.r / kBK;
+  if (a.r) {
+    VG_REQUIRE((reinterpret_cast<uintptr_t>(a.h) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.u) & 15) == 0 && a.ldh % 8 == 0,
+               "tapgemm_sm90: H and U must be 16-byte aligned, ldh a multiple of 8");
+    const uint64_t hdims[4] = {(uint64_t)a.r, (uint64_t)s.d1, 1, 1};
+    const uint64_t hstrides[3] = {(uint64_t)a.ldh * 2, (uint64_t)a.ldh * 2 * s.d1, (uint64_t)a.ldh * 2 * s.d1};
+    const uint32_t hbox[4] = {64, (uint32_t)s.box1, (uint32_t)s.box2, 1};
+    int rc = make_tmap_f16(&p.map_h, a.h, 4, hdims, hstrides, hbox);
+    if (rc) return rc;
+    const uint64_t udims[2] = {(uint64_t)a.r, (uint64_t)s.n};
+    const uint64_t ustrides[1] = {(uint64_t)a.r * 2};
+    const uint32_t ubox[2] = {64, (uint32_t)s.bn};
+    rc = make_tmap_f16(&p.map_u, a.u, 2, udims, ustrides, ubox);
     if (rc) return rc;
   }
   const int stage_bytes = kABytes + s.bn * kBK * 2;
@@ -287,7 +332,7 @@ int tapgemm_sm90_launch(const TapGemmArgs& a, cudaStream_t stream) {
   int grid = sm_count();
   if (grid > s.total_tiles) grid = s.total_tiles;
   if (grid < 1) return 0;
-  const int kind = (a.epi.geglu ? 1 : 0) | (a.epi.row_stats ? 2 : 0) | (a.epi.gelu ? 4 : 0) | (a.epi.relu ? 8 : 0);
+  const int kind = (a.epi.geglu ? 1 : 0) | (a.epi.row_stats ? 2 : 0) | (a.epi.gelu ? 4 : 0) | (a.epi.relu ? 8 : 0) | (a.r ? 16 : 0);
   switch (s.bn) {
     case 32: return launch_bn<32>(p, kind, grid, smem, stream);
     case 64: return launch_bn<64>(p, kind, grid, smem, stream);

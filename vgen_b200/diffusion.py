@@ -67,9 +67,10 @@ def cfg_forward(model, xt, ts, model_kwargs, by_keyword=False):
     layers so their epilogue overlaps a main loop.  Any other callable (e.g. a reference model) gets the reference's
     two separate calls.  VGEN_CFG_BATCH=0 disables the batching.
 
-    Keys a model names in `cfg_per_sample` are per-sample scalars (a number or a [b] tensor per branch, e.g. DreamVideo's
-    ag_strength): the two branches become one fp32 [2b] tensor, so branches with different values still run as one
-    forward, and one CUDA graph serves any value."""
+    Keys a model names in `cfg_per_sample` are per-sample values (a number or a [b] tensor per branch, e.g. DreamVideo's
+    ag_strength, or a [b, n] tensor, e.g. UNetSD_LoRA's lora_strength over n LoRA sets): the two branches become one fp32
+    [2b] (or [2b, n]) tensor, so branches with different values still run as one forward, and one CUDA graph serves any
+    value.  A number or [b] branch next to a [b, n] one is repeated over the n columns."""
     kc, ku = model_kwargs
     m = _unwrap(model)
     call = (lambda x, t, kw: model(x, t=t, **kw)) if by_keyword else (lambda x, t, kw: model(x, t, **kw))
@@ -79,7 +80,11 @@ def cfg_forward(model, xt, ts, model_kwargs, by_keyword=False):
         for k in kc:
             a, b = kc[k], ku[k]
             if k in per_sample and a is not None and b is not None:
-                merged[k] = torch.cat([_per_sample(a, xt), _per_sample(b, xt)])
+                pa, pb = _per_sample(a, xt), _per_sample(b, xt)
+                if pa.dim() != pb.dim():
+                    n = (pa if pa.dim() == 2 else pb).size(1)
+                    pa, pb = (p if p.dim() == 2 else p[:, None].expand(-1, n) for p in (pa, pb))
+                merged[k] = torch.cat([pa, pb])
             elif torch.is_tensor(a) and torch.is_tensor(b) and a.shape == b.shape and a.dtype == b.dtype and a.dim() >= 1 \
                     and a.size(0) == xt.size(0):
                 merged[k] = torch.cat([a, b], dim=0)
@@ -96,8 +101,14 @@ def cfg_forward(model, xt, ts, model_kwargs, by_keyword=False):
 
 
 def _per_sample(v, xt):
-    """A number or a 1- / b-entry tensor -> fp32 [b] on xt's device (b = xt.size(0))."""
-    t = torch.as_tensor(v, dtype=torch.float32).to(xt.device).reshape(-1)
+    """A number or a 1- / b-entry tensor -> fp32 [b] on xt's device (b = xt.size(0)); a 2-D [1 | b, n] tensor -> fp32
+    [b, n]."""
+    t = torch.as_tensor(v, dtype=torch.float32).to(xt.device)
+    if t.dim() == 2:
+        if t.size(0) not in (1, xt.size(0)):
+            raise ValueError(f"a per-sample [rows, n] argument must have 1 or {xt.size(0)} rows, got {t.size(0)}")
+        return t.expand(xt.size(0), t.size(1))
+    t = t.reshape(-1)
     if t.numel() not in (1, xt.size(0)):
         raise ValueError(f"a per-sample argument must be a number or have {xt.size(0)} entries, got {t.numel()}")
     return t.expand(xt.size(0))

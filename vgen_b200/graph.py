@@ -36,9 +36,10 @@ def enabled() -> bool:
 
 
 def _mode(owner):
-    """The module's numerics mode, part of every graph signature: a graph captured with one fp8_linear setting is never
-    replayed under the other (re-packing drops the graphs as well; this keeps the key honest on its own)."""
-    return (("fp8_linear", bool(getattr(owner, "fp8_linear", False))),)
+    """The module's numerics mode, part of every graph signature: a graph captured with one fp8_linear setting, or one runtime
+    LoRA layout (UNetSD_LoRA.lora_signature: the set names and ranks, not the strengths), is never replayed under another
+    (re-packing drops the graphs as well; this keeps the key honest on its own)."""
+    return (("fp8_linear", bool(getattr(owner, "fp8_linear", False))), ("lora", getattr(owner, "lora_signature", None)))
 
 
 class _Entry:

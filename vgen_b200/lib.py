@@ -47,6 +47,8 @@ _SIGNATURES = {
     "vgen_set_tapgemm_impl": [_i32],
     "vgen_set_tapgemm_bn": [_i32],
     "vgen_linear": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _EP, _vp],
+    "vgen_linear_lora": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _EP, _vp],
+    "vgen_lora_down": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i64, _vp, _i64, _i64, _vp],
     "vgen_linear_gelu_rowbias": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _i64, _vp],
     "vgen_adapter_condition": [_vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _f32, _i64, _vp, _i64, _vp],
     "vgen_conv2d_3x3": [_vp, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _EP, _vp],

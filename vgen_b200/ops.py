@@ -149,6 +149,58 @@ def linear(a, w, bias=None, residual=None, alpha=1.0, geglu=False, out=None, bn=
     return out
 
 
+def linear_lora(a, w, h, u, bias=None, residual=None, out=None, bn=0):
+    """out[m, n] = epi(a[m, k] @ w[n, k]^T + h[m, r] @ u[n, r]^T): a projection with the LoRA up projection as a K tail of
+    the same GEMM (one fp32 accumulator, one rounding).  h: lora_down's [m, r] output (r a multiple of 64), u: the up weights
+    [n, r].  `a` and `h` may be row-strided 2-D views."""
+    _chk16(a, "a"), _chk16(w, "w"), _chk16(h, "h"), _chk16(u, "u")
+    lead = a.shape[:-1]
+    a2, lda = _rows_view(a, "a")
+    h2, ldh = _rows_view(h, "h")
+    m, k = a2.shape
+    n, r = w.shape[0], u.shape[1]
+    if w.shape[1] != k or not w.is_contiguous():
+        raise _l.VgenError(f"linear_lora: weight {tuple(w.shape)} does not match k={k}")
+    if tuple(h2.shape) != (m, r) or u.shape[0] != n or not u.is_contiguous():
+        raise _l.VgenError(f"linear_lora: h {tuple(h2.shape)} / u {tuple(u.shape)} do not match m={m}, n={n}")
+    if out is None:
+        out = torch.empty(*lead, n, device=a.device, dtype=torch.float16)
+    o2, ldo = _rows_view(out, "out")
+    e, keep = _epilogue(n, bias, None, residual, 1.0, False, bn)
+    rc = _run("tapgemm", 2.0 * m * n * (k + r), 2.0 * (m * (k + r) + n * (k + r) + m * n),
+              lambda: _l.load().vgen_linear_lora(_p(a2), m, k, lda, _p(w), n, _p(h2), r, ldh, _p(u), _p(o2), ldo,
+                                                 ctypes.byref(e), _stream()),
+              tag=f"linear_lora m{m} k{k} r{r} n{n}{' res' if residual is not None else ''}")
+    _l.check(rc, "vgen_linear_lora")
+    return out
+
+
+def lora_down(x, d, col_set, col_scale, strength, rows_per_sample, r_pad, out=None):
+    """h[m, r_pad] = fp16(strength[row // rows_per_sample, col_set[j]] * col_scale[j] * x[row] . d[j]), zero past d's rows:
+    the LoRA down projection of every set and every projection reading x, with the per-sample strength [samples, sets]
+    (fp32 on the device) folded in."""
+    _chk16(x, "x"), _chk16(d, "d")
+    x2, ldx = _rows_view(x, "x")
+    m, k = x2.shape
+    r = d.shape[0]
+    if d.shape[1] != k or not d.is_contiguous():
+        raise _l.VgenError(f"lora_down: d {tuple(d.shape)} does not match k={k}")
+    if col_set.dtype != torch.int32 or col_scale.dtype != torch.float32 or col_set.numel() != r or col_scale.numel() != r:
+        raise _l.VgenError(f"lora_down: col_set must be int32 [{r}] and col_scale fp32 [{r}]")
+    if (strength.dtype != torch.float32 or strength.dim() != 2 or not strength.is_contiguous()
+            or strength.shape[0] * rows_per_sample < m or strength.device != x.device):
+        raise _l.VgenError(f"lora_down: strength must be contiguous fp32 [samples, sets] covering {m} rows")
+    if out is None:
+        out = torch.empty(m, r_pad, device=x.device, dtype=torch.float16)
+    o2, ldo = _rows_view(out, "out")
+    rc = _run("lora_down", 2.0 * m * r * k, 2.0 * (m * k + r * k + m * r_pad),
+              lambda: _l.load().vgen_lora_down(_p(x2), m, k, ldx, _p(d), r, _p(col_set), _p(col_scale), _p(strength),
+                                               strength.shape[1], int(rows_per_sample), _p(o2), ldo, int(r_pad), _stream()),
+              tag=f"m{m} k{k} r{r}")
+    _l.check(rc, "vgen_lora_down")
+    return out
+
+
 E4M3_MAX = 448.0
 
 

@@ -18,6 +18,7 @@ norm/softmax statistics, fp16 rounding where the reference materialises an fp16 
 from __future__ import annotations
 
 import os
+import re
 
 import torch
 
@@ -74,6 +75,8 @@ class _UNetBase(SpecModule):
     # FOLD_LN = True on a module followed by invalidate_packed(), turns it on; parity is the same (tests/test_gpu_parity.py).
     FOLD_LN = os.environ.get("VGEN_LN_FOLD", "0") == "1"
     _adapter_rows = None   # DreamVideo: (fp32 condition terms [groups, sum of hidden widths], frames per group) of the running forward
+    _lora_rt = False       # UNetSD_LoRA runtime LoRA: the base is packed unmerged and the pairs run as GEMM K tails
+    _lora_rows = None      # UNetSD_LoRA: (fp32 strengths [b, sets], b) of the running forward in runtime mode
 
     def __init__(self, config=None, in_dim=4, dim=512, y_dim=512, context_dim=512, hist_dim=156, dim_condition=4,
                  out_dim=6, num_tokens=4, dim_mult=[1, 2, 3, 4], num_heads=None, head_dim=64, num_res_blocks=3,
@@ -207,12 +210,16 @@ class _UNetBase(SpecModule):
             gw, gb = sd[p + "ff.net.0.proj.weight"].detach().float(), sd[p + "ff.net.0.proj.bias"].detach().float()
             bn = _geglu_bn_fp8(gw.shape[0]) if q8 else _geglu_bn(gw.shape[0])
             if ln_fold:
-                # norm1 -> attn1.qkv, norm2 -> attn2.q (cross) / attn2.qkv, norm3 -> GEGLU projection
-                fold(a1 + "qkv", torch.cat([sd[a1 + "to_q.weight"], sd[a1 + "to_k.weight"], sd[a1 + "to_v.weight"]], 0), None, p + "norm1.")
-                if cross:
-                    fold(a2 + "q", sd[a2 + "to_q.weight"], None, p + "norm2.")
-                else:
-                    fold(a2 + "qkv", torch.cat([sd[a2 + "to_q.weight"], sd[a2 + "to_k.weight"], sd[a2 + "to_v.weight"]], 0), None, p + "norm2.")
+                # norm1 -> attn1.qkv, norm2 -> attn2.q (cross) / attn2.qkv, norm3 -> GEGLU projection; not into the projections
+                # a runtime LoRA adapts: the epilogue's row statistics would scale the LoRA tail too
+                if not self._lora_rt:
+                    fold(a1 + "qkv", torch.cat([sd[a1 + "to_q.weight"], sd[a1 + "to_k.weight"], sd[a1 + "to_v.weight"]], 0), None,
+                         p + "norm1.")
+                    if cross:
+                        fold(a2 + "q", sd[a2 + "to_q.weight"], None, p + "norm2.")
+                    else:
+                        fold(a2 + "qkv", torch.cat([sd[a2 + "to_q.weight"], sd[a2 + "to_k.weight"], sd[a2 + "to_v.weight"]], 0),
+                             None, p + "norm2.")
                 g3, b3 = sd[p + "norm3.weight"].detach().float(), sd[p + "norm3.bias"].detach().float()
                 gb = gb + gw @ b3
                 gw = gw * g3[None, :]
@@ -383,13 +390,29 @@ class _UNetBase(SpecModule):
                            residual=hcur.view(b, f, h * w, L.cout) if last else None).view(hcur.shape)
         return t
 
-    @staticmethod
-    def _ln_linear(t, W, key, nrm):
+    def _ln_linear(self, t, W, key, nrm):
         """nn.LayerNorm `nrm` followed by the bias-free projection `key` (util.py:694-704): when the pack folded the norm into
         the weights (key.cs present) only the row statistics are computed and the GEMM epilogue applies them."""
         if key + ".cs" in W:
             return ops.linear(t, W[key], bias=W[key + ".lb"], ln=(ops.row_stats(t), W[key + ".cs"]))
-        return _UNetBase._proj(ops.layer_norm(t, W[nrm + "g"], W[nrm + "b"]), W, key)
+        xn = ops.layer_norm(t, W[nrm + "g"], W[nrm + "b"])
+        lo = self._lora_site(W, key)
+        if lo is not None:
+            return self._lora_linear(xn, W, key, lo)
+        return _UNetBase._proj(xn, W, key)
+
+    def _lora_site(self, W, key):
+        """The runtime LoRA operands of the packed projection `key` in the running forward, or None."""
+        if self._lora_rows is None:
+            return None
+        return W["__lora__"].get(key)
+
+    def _lora_linear(self, x, W, key, lo, **kw):
+        """x W[key]^T + sum over sets j of strength[sample, j] * alpha_j / rank_j * (x D_j^T) U_j^T: the down projections of
+        every set in one launch (ops.lora_down, strength folded in), the up projections as the K tail of the projection's GEMM."""
+        strength, b = self._lora_rows
+        h = ops.lora_down(x, lo["d"], lo["set"], lo["scale"], strength, x.shape[0] // b, lo["rpad"])
+        return ops.linear_lora(x, W[key], h, lo["u"], **kw)
 
     def _self_attn_qkv_spatial(self, t, W, p, nrm, n, hw, inner):
         qkv = self._ln_linear(t, W, p + "qkv", nrm)             # [M, 3*inner]
@@ -404,6 +427,9 @@ class _UNetBase(SpecModule):
         t' = t + sublayer(t).  Without one it is the plain projection with the residual."""
         ad = W.get(p + mod)
         if ad is None:
+            lo = self._lora_site(W, p + out + "w")
+            if lo is not None:
+                return self._lora_linear(produce(None).view(-1, width), W, p + out + "w", lo, bias=W[p + out + "b"], residual=t)
             return self._proj(produce(None).view(-1, width), W, p + out + "w", bias=W[p + out + "b"], residual=t)
         if ad["pos"] == "serial":
             t = self._proj(produce(None).view(-1, width), W, p + out + "w", bias=W[p + out + "b"], residual=t)
@@ -451,7 +477,9 @@ class _UNetBase(SpecModule):
             kv, div = self._frame_kv(*ctx_tokens, W[p + "attn2.kv"], f), 1
         else:
             bctx, lctx, cdim = ctx_tokens.shape
-            kv, div = ops.linear(ctx_tokens.view(-1, cdim), W[p + "attn2.kv"]).view(bctx, lctx, 2 * inner), f
+            c2, lo = ctx_tokens.view(-1, cdim), self._lora_site(W, p + "attn2.kv")
+            kv = ops.linear(c2, W[p + "attn2.kv"]) if lo is None else self._lora_linear(c2, W, p + "attn2.kv", lo)
+            kv, div = kv.view(bctx, lctx, 2 * inner), f
         t = self._sublayer_out(t, W, p, "cross_attn_adapter", "attn2.to_out.0.", inner, hw, lambda o: ops.attention_d64(
             q, kv[:, :, :inner], kv[:, :, inner:], heads, kv_batch_div=div, out=None if o is None else o.view(n, hw, inner)))
         return self._feed_forward(t, W, p, hw)
@@ -586,6 +614,16 @@ class _UNetBase(SpecModule):
             return t
         return ops.cp_to_pc(t.contiguous().view(b * L, c, 1).float(), b * L, c, 1).view(b, L, c)
 
+    def add_lora(self, name, state_dict, alpha=None):
+        raise NotImplementedError(f"vgen_b200 {type(self).__name__}: runtime LoRA sets exist on UNetSD_LoRA only")
+
+    def remove_lora(self, name):
+        raise NotImplementedError(f"vgen_b200 {type(self).__name__}: runtime LoRA sets exist on UNetSD_LoRA only")
+
+    def _refuse_lora(self, kwargs):
+        if "lora_strength" in kwargs:
+            raise NotImplementedError(f"vgen_b200 {type(self).__name__}: lora_strength is a UNetSD_LoRA argument")
+
     def _check_x(self, x, t):
         if not x.is_cuda:
             raise ops._l.VgenError("vgen_b200 UNet: inputs must be CUDA tensors (no CPU path exists)")
@@ -603,6 +641,7 @@ class UNetSD_T2VBase(_UNetBase):
     @torch.no_grad()
     def forward(self, x, t, y=None, fps=None, masked=None, video_mask=None, focus_present_mask=None,
                 prob_focus_present=0., mask_last_frame_num=0, **kwargs):
+        self._refuse_lora(kwargs)
         self._check_x(x, t)
         W = self._packed or self._pack()
         b, c, f, h, w = x.shape
@@ -658,6 +697,7 @@ class UNetSD_I2VGen(_UNetBase):
     @torch.no_grad()
     def forward(self, x, t, y=None, image=None, local_image=None, masked=None, fps=None, video_mask=None,
                 focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0, **kwargs):
+        self._refuse_lora(kwargs)
         self._check_x(x, t)
         if local_image is None or fps is None:
             raise ValueError("UNetSD_I2VGen.forward needs local_image and fps")
@@ -763,6 +803,7 @@ class UNetSD_VideoLCM(_UNetBase):
     def forward(self, x, t, y=None, depth=None, image=None, motion=None, local_image=None, single_sketch=None,
                 masked=None, canny=None, sketch=None, histogram=None, fps=None, video_mask=None,
                 focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0, **kwargs):
+        self._refuse_lora(kwargs)
         self._check_x(x, t)
         name = type(self).__name__
         conds = dict(depth=depth, local_image=local_image, motion=motion, canny=canny, sketch=sketch,
@@ -876,6 +917,7 @@ class UNetSD_DreamVideo(_UNetBase):
     @torch.no_grad()
     def forward(self, x, t, y=None, y_image=None, fps=None, masked=None, video_mask=None, focus_present_mask=None,
                 prob_focus_present=0., mask_last_frame_num=0, ag_strength=1, **kwargs):
+        self._refuse_lora(kwargs)
         self._check_x(x, t)
         b, c, f, h, w = x.shape
         cond = self._condition_rows(y_image, ag_strength, b, f)
@@ -912,12 +954,24 @@ class UNetSD_LoRA(_UNetBase):
     (:161-195).  The state_dict keeps the LoRA pairs (2 008 tensors at the released rank 4, 1 480 without LoRA), so strict
     loading and get_lora_merged_model (inference_instructvideo_entrance.py:301-353) work unchanged.
 
-    The forward never runs the pairs: the pack folds each one into the projection it adapts, W + s * up @ down with
+    Merged mode (the default): the pack folds each pair into the projection it adapts, W + s * up @ down with
     s = lora_alpha / lora_rank (1 when lora_alpha is None), the merge the reference's inference performs, computed in fp64
     on the host and rounded to the masters' dtype (merged_state_dict).  The packed weights are then exactly
-    UNetSD_T2VBase's for the merged dict, and the LoRA costs nothing per step.  fps is ignored and y is required, as in the
-    reference (:1315-1316)."""
+    UNetSD_T2VBase's for the merged dict, and the LoRA costs nothing per step.
+
+    Runtime mode: entered by the first add_lora() or the first forward with lora_strength (one re-pack of the base,
+    unmerged).  Every LoRA set -- the model's own pairs as set 0, "default", when use_lora=True, then the added ones in
+    order (lora_names) -- stays in a separate fp16 arena; set j on sample i adds lora_strength[i, j] * alpha_j / rank_j *
+    U_j D_j x to each of the 4 projections of every attention.  Per projection input one launch computes the down
+    projections of all sets (strength folded in, ops.lora_down) and the up projections run as the K tail of the projection's
+    own GEMM (ops.linear_lora).  lora_strength, a keyword of the call (forward keeps the reference's signature), is a number,
+    a [b] tensor or a [b, len(lora_names)] tensor; without it every set runs at 1.  Strength values never enter a CUDA graph's signature, the set layout does.  fp8_linear is refused in
+    runtime mode.
+
+    fps is ignored and y is required, as in the reference (:1315-1316)."""
     KIND = "t2v"
+    cfg_per_sample = ("lora_strength",)
+    _LORA_KEY = re.compile(r"^(.*\.)(to_(?:q|k|v|out)_lora)\.(down|up)_linear\.weight$")
 
     def __init__(self, in_dim=7, dim=512, y_dim=512, context_dim=512, out_dim=6, dim_mult=[1, 2, 3, 4], num_heads=None,
                  head_dim=64, num_res_blocks=3, attn_scales=[1 / 2, 1 / 4, 1 / 8], use_scale_shift_norm=True, dropout=0.1,
@@ -937,10 +991,183 @@ class UNetSD_LoRA(_UNetBase):
         self.use_lora, self.lora_rank, self.lora_alpha = use_lora, lora_rank, lora_alpha
         # get_lora_merged_model's alpha (inference_instructvideo_entrance.py:315)
         self.lora_scale = lora_alpha / lora_rank if (lora_alpha is not None and self._lora_rank) else 1.0
+        self._lora_added = {}   # name -> ({attention prefix + LoRA module: (down, up) fp16}, rank, alpha / rank)
 
     def _plan_kwargs(self, config):
         return dict(lora_rank=self._lora_rank)
 
+    # ------------------------------------------------------------------------------ runtime LoRA sets
+    @property
+    def lora_names(self):
+        """The LoRA sets in strength-column order: "default" (the model's own pairs, use_lora=True), then the added sets."""
+        return (["default"] if self.plan.lora_rank else []) + list(self._lora_added)
+
+    @property
+    def lora_signature(self):
+        """Part of every CUDA graph signature (graph.py): the mode and the set layout, never the strengths."""
+        if not self._lora_rt:
+            return None
+        ranks = ([self.plan.lora_rank] if self.plan.lora_rank else []) + [r for _, r, _ in self._lora_added.values()]
+        return tuple(zip(self.lora_names, ranks))
+
+    @_UNetBase.fp8_linear.setter
+    def fp8_linear(self, value):
+        if value is True and self._lora_rt:
+            raise NotImplementedError("vgen_b200 UNetSD_LoRA: fp8_linear together with runtime LoRA is not supported")
+        _UNetBase.fp8_linear.fset(self, value)
+
+    def _attention_prefixes(self, sd):
+        return sorted(k[:-len("to_q.weight")] for k in sd if k.endswith(("attn1.to_q.weight", "attn2.to_q.weight")))
+
+    def add_lora(self, name, state_dict, alpha=None):
+        """Add a LoRA set: the *.to_{q,k,v,out}_lora.{down,up}_linear.weight pairs of every attention (unet_lora.py:114-159)
+        from a full InstructVideo checkpoint or a LoRA-only dict, one rank (1 to 64) for all of them, applied at alpha / rank
+        (1 when alpha is None).  Switches the model to runtime mode; the base weights are not touched."""
+        if not isinstance(name, str) or not name:
+            raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: the name must be a non-empty string, got {name!r}")
+        if name in self.lora_names:
+            raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: a LoRA set named {name!r} exists already")
+        if alpha is not None and (isinstance(alpha, bool) or not isinstance(alpha, (int, float)) or not torch.isfinite(
+                torch.tensor(float(alpha)))):
+            raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: alpha must be a finite number or None, got {alpha!r}")
+        if self._fp8:
+            raise NotImplementedError("vgen_b200 UNetSD_LoRA: fp8_linear together with runtime LoRA is not supported")
+        base = self.state_dict()
+        atts = self._attention_prefixes(base)
+        expected = {f"{a}{mod}.{d}_linear.weight" for a in atts for mod, _ in arch.LORA_SITES for d in ("down", "up")}
+        got = {k for k in state_dict if self._LORA_KEY.match(k)}
+        missing, extra = sorted(expected - got), sorted(got - expected)
+        if missing:
+            raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: set {name!r} lacks {len(missing)} of the {len(expected)} LoRA "
+                             f"weights, first {missing[0]}")
+        if extra:
+            raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: set {name!r} has LoRA weights this model has no site for, "
+                             f"first {extra[0]}")
+        rank, pairs = None, {}
+        for a in atts:
+            for mod, target in arch.LORA_SITES:
+                kd, ku = f"{a}{mod}.down_linear.weight", f"{a}{mod}.up_linear.weight"
+                d, u, w = state_dict[kd], state_dict[ku], base[a + target]
+                if (not torch.is_tensor(d) or not torch.is_tensor(u) or d.dim() != 2 or u.dim() != 2
+                        or d.shape[1] != w.shape[1] or u.shape[0] != w.shape[0] or u.shape[1] != d.shape[0]):
+                    raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: set {name!r}: {kd} / {ku} have shapes "
+                                     f"{tuple(getattr(d, 'shape', ()))} / {tuple(getattr(u, 'shape', ()))}, the site "
+                                     f"{a + target} needs [r, {w.shape[1]}] / [{w.shape[0]}, r]")
+                r = d.shape[0]
+                if not 1 <= r <= 64:
+                    raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: set {name!r}: {kd} has rank {r}, supported 1 to 64")
+                if rank is not None and r != rank:
+                    raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: set {name!r}: {kd} has rank {r}, the set's other "
+                                     f"pairs {rank}; a set has one rank")
+                rank = r
+                d16 = d.detach().to(device="cpu", dtype=torch.float16)
+                u16 = u.detach().to(device="cpu", dtype=torch.float16)
+                for key, t in ((kd, d16), (ku, u16)):
+                    if not bool(torch.isfinite(t).all()):
+                        raise ValueError(f"vgen_b200 UNetSD_LoRA.add_lora: set {name!r}: {key} has values that are not "
+                                         "finite in fp16")
+                pairs[a + mod] = (d16, u16)
+        self._lora_added[name] = (pairs, rank, float(alpha) / rank if alpha is not None else 1.0)
+        self._lora_changed()
+
+    def remove_lora(self, name):
+        """Remove an added LoRA set (the model's own "default" pairs belong to its state_dict and stay)."""
+        if name not in self._lora_added:
+            raise ValueError(f"vgen_b200 UNetSD_LoRA.remove_lora: no added LoRA set named {name!r} "
+                             f"(added: {list(self._lora_added)})")
+        del self._lora_added[name]
+        self._lora_changed()
+
+    def _enter_runtime(self):
+        if self._fp8:
+            raise NotImplementedError("vgen_b200 UNetSD_LoRA: fp8_linear together with runtime LoRA is not supported")
+        if not self._lora_rt:
+            self._lora_rt = True
+            self.invalidate_packed()        # one re-pack of the base, unmerged
+
+    def _lora_changed(self):
+        """A set was added or removed: rebuild the LoRA arena (and drop the graphs that read it), keep the base arena."""
+        if not self._lora_rt:
+            self._enter_runtime()
+        elif self._packed is not None:
+            self._packed.pop("__lora__", None)
+            self._packed.pop("__graphs__", None)
+
+    def _lora_arena(self, W):
+        """Per packed projection a LoRA adapts: d [R, k] (the down weights of every set and every projection fused into it),
+        u [n, R'] (the up weights, block-diagonal over q / k / v, R' = R padded to the next multiple of 64), the set and
+        alpha / rank of each column.  Column order: projection, then set."""
+        sets = []
+        if self.plan.lora_rank:
+            sd = self.state_dict()
+            sets.append((lambda site, sd=sd: (sd[site + ".down_linear.weight"], sd[site + ".up_linear.weight"]),
+                         self.plan.lora_rank, self.lora_scale))
+        sets += [(lambda site, pairs=pairs: pairs[site], r, sc) for pairs, r, sc in self._lora_added.values()]
+        if not sets:
+            return {}
+        dev, arena = self.device, {}
+        for att in self._attention_prefixes(self.state_dict()):
+            groups = [(att + "qkv", ("to_q_lora", "to_k_lora", "to_v_lora"))] if att + "qkv" in W else \
+                [(att + "q", ("to_q_lora",)), (att + "kv", ("to_k_lora", "to_v_lora"))]
+            for key, mods in groups + [(att + "to_out.0.w", ("to_out_lora",))]:
+                downs, ups, cset, cscale = [], [], [], []
+                for mod in mods:
+                    for j, (pair, r, sc) in enumerate(sets):
+                        d, u = pair(att + mod)
+                        downs.append(d.detach().double().cpu())
+                        ups.append(u.detach().double().cpu())
+                        cset += [j] * r
+                        cscale += [sc] * r
+                rtot = len(cset)
+                rpad = -(-rtot // 64) * 64
+                n_mod = ups[0].shape[0]
+                u_cat = torch.zeros(n_mod * len(mods), rpad, dtype=torch.float64)
+                col = 0
+                for i, u in enumerate(ups):
+                    mi = i // len(sets)
+                    u_cat[mi * n_mod:(mi + 1) * n_mod, col:col + u.shape[1]] = u
+                    col += u.shape[1]
+                arena[key] = {"d": _f16(torch.cat(downs), dev), "u": _f16(u_cat, dev), "rpad": rpad,
+                              "set": torch.tensor(cset, dtype=torch.int32, device=dev),
+                              "scale": torch.tensor(cscale, dtype=torch.float32, device=dev)}
+        return arena
+
+    def _strength_rows(self, lora_strength, x):
+        """lora_strength -> fp32 [b, len(lora_names)] on x's device (None: merged mode, or no set), validated before the
+        model enters runtime mode."""
+        b = x.shape[0]
+        n = len(self.lora_names)
+        if lora_strength is None:
+            if not self._lora_rt or not n:
+                return None
+            return torch.ones(b, n, device=x.device, dtype=torch.float32)
+        if not n:
+            raise ValueError("vgen_b200 UNetSD_LoRA: lora_strength was given but the model has no LoRA set "
+                             "(use_lora=False and nothing added with add_lora)")
+        if self._fp8:
+            raise NotImplementedError("vgen_b200 UNetSD_LoRA: fp8_linear together with runtime LoRA is not supported")
+        if torch.is_tensor(lora_strength):
+            s = lora_strength.detach().to(device=x.device, dtype=torch.float32)
+            if s.dim() == 0:
+                s = s.reshape(1, 1).expand(b, n)
+            elif s.dim() == 1 and s.shape[0] == b:
+                s = s[:, None].expand(b, n)
+            elif not (s.dim() == 2 and tuple(s.shape) == (b, n)):
+                raise ValueError(f"vgen_b200 UNetSD_LoRA: lora_strength must be a number, a [{b}] tensor or a [{b}, {n}] "
+                                 f"tensor (sets {self.lora_names}), got {tuple(lora_strength.shape)}")
+            if not bool(torch.isfinite(s).all()):
+                raise ValueError("vgen_b200 UNetSD_LoRA: lora_strength has non-finite values")
+            s = s.contiguous()
+        elif isinstance(lora_strength, (int, float)) and not isinstance(lora_strength, bool):
+            if not torch.isfinite(torch.tensor(float(lora_strength))):
+                raise ValueError(f"vgen_b200 UNetSD_LoRA: lora_strength must be finite, got {lora_strength!r}")
+            s = torch.full((b, n), float(lora_strength), device=x.device, dtype=torch.float32)
+        else:
+            raise ValueError(f"vgen_b200 UNetSD_LoRA: lora_strength must be a number or a tensor, got {lora_strength!r}")
+        self._enter_runtime()
+        return s
+
+    # ------------------------------------------------------------------------------ weight packing / forward
     def merged_state_dict(self):
         """state_dict() with every LoRA pair folded into its projection (W + lora_scale * up @ down in fp64, rounded to W's
         dtype) and the LoRA keys dropped: the UNetSD_T2VBase / use_lora=False layout.  Without LoRA it is state_dict()."""
@@ -959,21 +1186,53 @@ class UNetSD_LoRA(_UNetBase):
         return out
 
     def _pack_state_dict(self):
+        if self._lora_rt:   # runtime mode: the base unmerged, the pairs live in the LoRA arena
+            return {k: v for k, v in self.state_dict().items() if "_lora." not in k}
         return self.merged_state_dict()
 
     @graphed
     @torch.no_grad()
-    def forward(self, x, t, y, fps=None, video_mask=None, focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0):
+    def forward(self, x, t, y, fps=None, video_mask=None, focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0,
+                lora_strength=None):
         self._check_x(x, t)
         if y is None:
             raise ValueError("UNetSD_LoRA.forward needs y (the reference has no zero_y fallback)")
         W = self._packed or self._pack()
+        if self._lora_rt and "__lora__" not in W:
+            W["__lora__"] = self._lora_arena(W)
         b, c, f, h, w = x.shape
         emb = self._time_embedding(t, None, W)                        # fps is ignored (unet_lora.py:1315)
         ctx = self._to_f16_rows(y)
         xin = ops.cp_to_pc(x.contiguous(), b, c, f * h * w, c_pad=8).view(b * f, h, w, 8)
-        out = self._trunk(xin, emb, ctx, W, b, f)                     # [(b f), h, w, out_dim]
+        self._lora_rows = (lora_strength, b) if lora_strength is not None else None
+        try:
+            out = self._trunk(xin, emb, ctx, W, b, f)                 # [(b f), h, w, out_dim]
+        finally:
+            self._lora_rows = None
         return ops.pc_to_cp(out.view(b, f * h * w, self.out_dim), b, self.out_dim, f * h * w).view(b, self.out_dim, f, h, w)
+
+    _forward_graphed = forward
+
+    def forward(self, x, t, y, fps=None, video_mask=None, focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0):
+        """The reference's forward signature; in runtime mode every LoRA set runs at strength 1.  Per-sample strengths are a
+        keyword of the call, model(x, t, y, lora_strength=...) (__call__)."""
+        return self._forward_graphed(x, t, y, fps, video_mask, focus_present_mask, prob_focus_present, mask_last_frame_num,
+                                     lora_strength=self._strength_rows(None, x))
+
+    def __call__(self, *args, lora_strength=None, **kwargs):
+        if lora_strength is None:
+            return super().__call__(*args, **kwargs)
+        # validated here, outside any graph capture (the finiteness check reads the strengths on the host)
+        s = self._strength_rows(lora_strength, args[0] if args else kwargs["x"])
+        return self._forward_graphed(*args, lora_strength=s, **kwargs)
+
+    def _forward_eager(self, x, t, y, fps=None, video_mask=None, focus_present_mask=None, prob_focus_present=0.,
+                       mask_last_frame_num=0, lora_strength=None):
+        return UNetSD_LoRA._forward_graphed.__wrapped_eager__(
+            self, x, t, y, fps, video_mask, focus_present_mask, prob_focus_present, mask_last_frame_num,
+            lora_strength=self._strength_rows(lora_strength, x))
+
+    forward.__wrapped_eager__ = _forward_eager
 
 
 class UNetSD_SR600(_UNetBase):
@@ -1002,6 +1261,7 @@ class UNetSD_SR600(_UNetBase):
     @torch.no_grad()
     def forward(self, x, t, y, x_lr=None, fps=None, video_mask=None, focus_present_mask=None, prob_focus_present=0.,
                 mask_last_frame_num=0, **kwargs):
+        self._refuse_lora(kwargs)
         self._check_x(x, t)
         W = self._packed or self._pack()
         b, c, f, h, w = x.shape
@@ -1066,6 +1326,7 @@ class UNetSD_HiGen(_UNetBase):
     @torch.no_grad()
     def forward(self, x, t, y=None, fps=None, masked=None, video_mask=None, spat_prior=None, motion_cond=None,
                 appearance_cond=None, focus_present_mask=None, prob_focus_present=0., mask_last_frame_num=0, **kwargs):
+        self._refuse_lora(kwargs)
         self._check_x(x, t)
         if y is None or spat_prior is None or motion_cond is None or appearance_cond is None:
             raise ValueError("UNetSD_HiGen.forward needs y, spat_prior, motion_cond and appearance_cond")
